@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — the per-update mixing hot path on B200 (BASELINE.json metric:
+"""bench.py — the per-update mixing hot path on H100 (BASELINE.json metric:
 "real-time HRTF voices @48kHz/1024-sample update; samples/sec mixed").
 
 A step = ONE 1024-frame mix update of the whole voice set (the voice loop of
@@ -13,6 +13,7 @@ same voices.
 
   python bench.py --gpus N --steps K --warmup W            # the CUDA mixer (libb200mix.so)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's own CPU mixer
+  python bench.py ... --dump-outputs DIR    # also writes the last timed update's RealOut block
 
 value  : voice-samples/s with everything resident in HBM, device-timed (CUDA events on the
          mixer's stream around each update incl. the RealOut reduce, L2 flushed between
@@ -47,7 +48,8 @@ WORKLOAD = ("config2: 4096 mono 48k voices per GPU, Default HRTF 64-tap HRIR pai
             "bsinc24, pitch U[0.5,2) (1/16 at 1.0)")
 METRIC = "voice-samples/s mixed (HRTF, bsinc24, 1024-frame updates)"
 SUSTAINED_VOICES = 131072
-NUM_SMS, FP32_LANES = 148, 128
+FP32_LANES = 128                     # FP32 lanes per SM (Hopper)
+HBM_GBS_DATASHEET = 3350.0           # H100 SXM data sheet
 
 
 # --------------------------------------------------------------------------- helpers
@@ -328,6 +330,17 @@ def main_reference(args):
 
 
 # --------------------------------------------------------------------------- CUDA arm
+def dump_real_out(torch, ptr, out_dir):
+    """Copies the [2][1024] float RealOut block b200mix_render_device left at device address
+    `ptr` to out_dir/real_out.npy (float32)."""
+    class _Block:
+        __cuda_array_interface__ = {"shape": (2, FRAMES), "typestr": "<f4", "data": (ptr, False),
+                                    "strides": None, "version": 2}
+    out = torch.as_tensor(_Block(), device="cuda").cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "real_out.npy"), out)
+
+
 class Mixer:
     """One b200mix device holding the scene voices `indices` (global indices) as local voices."""
 
@@ -468,12 +481,13 @@ def main_cuda(args):
             dist.barrier()
         torch.cuda.synchronize()
 
-    def timed_device_steps(steps, warmup):
+    def timed_device_steps(steps, warmup, dump=None):
         """K device-timed updates: events on the mixer's stream around every update, L2 flushed
         before each, the K updates enqueued back to back and the host synchronised once at the end
         (the contract's bracket) — a per-update host round trip would put host wake-up jitter of
         the slowest of N processes into every rank-0 reduce.  A short host-synchronous pass
         afterwards samples the per-kernel / per-collective device times.
+        With `dump` (rank 0), the RealOut block of the last timed update is written there.
         Returns (per-step ms, per-step voice-kernel ms, per-step reduce us, launches)."""
         for _ in range(warmup):
             mx.render_device()
@@ -491,6 +505,8 @@ def main_cuda(args):
             evs.append((e0, e1))
         torch.cuda.synchronize()
         launches = lib.b200mix_launch_count(h) - l0
+        if dump and rank == 0:
+            dump_real_out(torch, mx.out_ptr.value, dump)
         step_ms = [a.elapsed_time(b) for a, b in evs]
         mix_ms, red_us = [], []
         ru = C.c_float(-1.0)
@@ -529,7 +545,7 @@ def main_cuda(args):
     clocks = ClockSampler(local)
     if rank == 0:
         clocks.start()
-    step_ms, mix_ms, red_us, launches = timed_device_steps(args.steps, args.warmup)
+    step_ms, mix_ms, red_us, launches = timed_device_steps(args.steps, args.warmup, args.dump_outputs)
     lib.b200mix_profile(h, 0)
     alg_flops = algorithmic_flops(lib, h, mx.params, nv)
     t_total = max_over_ranks(float(np.sum(step_ms)))
@@ -611,28 +627,20 @@ def main_cuda(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "MEASURED_PEAKS.json hbm_gbs (burst copy)" if peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", HBM_GBS_DATASHEET))
+        peak_src = ("MEASURED_PEAKS.json hbm_gbs (burst copy)" if peaks
+                    else f"H100 SXM data sheet {HBM_GBS_DATASHEET:.0f} GB/s")
         mean_pitch = float(np.mean(mx.pitches))
         alg_bytes = algorithmic_bytes_per_voice(mean_pitch) * nv
         good = [m for m in mix_ms if m > 0]
         mix_avg = float(np.mean(good)) if good else None
         achieved = alg_bytes / (mix_avg * 1e-3) / 1e9 if mix_avg else None
-        ncu = {}
-        try:
-            ncu = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))["k_mix_voices"]
-        except Exception:
-            pass
-        traffic = ncu.get("dram_bytes_per_launch")
-        sm_max = float((clk or {}).get("sm_max_mhz") or peaks.get("sm_max_mhz", 1965.0))
-        fp32_peak = NUM_SMS * FP32_LANES * 2 * sm_max * 1e6 / 1e12           # TFLOP/s
+        num_sms = torch.cuda.get_device_properties(local).multi_processor_count
+        sm_max = float((clk or {}).get("sm_max_mhz") or peaks.get("sm_max_mhz", 1980.0))
+        fp32_peak = num_sms * FP32_LANES * 2 * sm_max * 1e6 / 1e12           # TFLOP/s
         fp32_ach = alg_flops / (mix_avg * 1e-3) / 1e12 if (mix_avg and alg_flops) else None
-        wav = ncu.get("smem_wavefronts_per_launch")
-        smem_peak = NUM_SMS * sm_max * 1e6                                     # wavefronts/s (1 per clk per SM)
-        smem_ach = wav / (mix_avg * 1e-3) if (wav and mix_avg) else None
         fracs = {"hbm": (achieved / peak) if achieved else None,
-                 "fp32": (fp32_ach / fp32_peak) if fp32_ach else None,
-                 "smem": (smem_ach / smem_peak) if smem_ach else None}
+                 "fp32": (fp32_ach / fp32_peak) if fp32_ach else None}
         bound = max((k for k in fracs if fracs[k] is not None), key=lambda k: fracs[k], default="hbm")
         line = {
             "metric": METRIC,
@@ -655,23 +663,19 @@ def main_cuda(args):
                               + ("; the RealOut reduce is inside b200mix_render and rank 0's host buffer "
                                  "receives the summed block" if world > 1 else "")},
             "gpu_launches": int(launches),
+            "gpu": torch.cuda.get_device_name(local),
             "clocks": clk,
             "roofline": {"bound": bound, "kernel": "k_mix_voices",
                          "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": fracs["hbm"],
-                         "traffic": traffic, "traffic_source": ncu.get("source"),
                          "peak_source": peak_src,
                          "kernel_ms": mix_avg, "algorithmic_bytes_per_launch": alg_bytes,
                          "fp32": {"achieved": fp32_ach, "peak": fp32_peak, "unit": "TFLOP/s", "frac": fracs["fp32"],
                                   "algorithmic_flops_per_launch": alg_flops,
-                                  "peak_source": f"{NUM_SMS} SMs x {FP32_LANES} lanes x 2 x {sm_max:.0f} MHz"},
-                         "smem": {"achieved": smem_ach, "peak": smem_peak, "unit": "wavefronts/s",
-                                  "frac": fracs["smem"], "wavefronts_per_launch": wav,
-                                  "source": ncu.get("source"),
-                                  "peak_source": f"{NUM_SMS} SMs x 1 wavefront/clk x {sm_max:.0f} MHz"},
-                         "note": "frac is the contract's algorithmic-bytes/HBM figure; an HRTF voice is "
-                                 "~100 flop/B, so the kernel is bounded by shared-memory wavefronts and FP32 "
-                                 "issue (sub-records), not by HBM — `bound` names the highest fraction"},
+                                  "peak_source": f"{num_sms} SMs x {FP32_LANES} lanes x 2 x {sm_max:.0f} MHz"},
+                         "note": "frac is the algorithmic-bytes/HBM figure; an HRTF voice is ~100 flop/B, "
+                                 "so the kernel is bounded by shared-memory traffic and FP32 issue, not by "
+                                 "HBM — `bound` names the higher of the two fractions"},
         }
         if collective:
             line["collective"] = collective
@@ -747,6 +751,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sustained", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed update's RealOut block as DIR/real_out.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         main_reference(args)

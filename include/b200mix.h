@@ -1,4 +1,4 @@
-/* b200mix.h — C ABI of the Blackwell (sm_100a) mixer backend for OpenAL Soft.
+/* b200mix.h — C ABI of the Hopper (sm_90a) mixer backend for OpenAL Soft.
  *
  * This is the drop-in boundary: one level above the reference's per-kernel
  * function pointers, it replaces the body of DeviceBase::renderSamples(unsigned)

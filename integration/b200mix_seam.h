@@ -1,4 +1,4 @@
-/* b200mix_seam.h — the seam a maintainer adds to OpenAL Soft to mix on a B200 through
+/* b200mix_seam.h — the seam a maintainer adds to OpenAL Soft to mix on an H100 through
  * libb200mix.so (include/b200mix.h).  Declared here, called from the patched places of
  * alc/alu.cpp (integration/alu_seam.patch), alc/effects/convolution.cpp
  * (integration/convolution_seam.patch) and core/device.cpp (integration/device_seam.patch),

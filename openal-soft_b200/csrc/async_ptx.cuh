@@ -1,6 +1,6 @@
-// async_ptx.cuh — thin wrappers over the sm_100a asynchronous-copy and tensor-core PTX the
+// async_ptx.cuh — thin wrappers over the sm_90a asynchronous-copy and tensor-core PTX the
 // kernels use: mbarrier, the bulk ("1-D TMA") global->shared copy cp.async.bulk (SASS: UBLKCP),
-// tcgen05 tensor-memory allocation / MMA / load (SASS: UTCxMMA, LDTM).
+// the warpgroup MMA wgmma.mma_async (SASS: HGMMA).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -42,52 +42,29 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
 __device__ __forceinline__ void fence_proxy_async_smem()
 { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tcgen05: tensor memory and the 5th-generation MMA -------------------------------------
-template<uint32_t COLS> __device__ __forceinline__ void tmem_alloc(uint32_t *slot_in_smem)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-        :: "r"(smem_u32(slot_in_smem)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template<uint32_t COLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr)
-{ asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory"); }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor), no swizzle ("interleave"):
-// start address, leading / stride byte offsets (all >> 4), version 1 (Blackwell).
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes)
+// ---- wgmma: Hopper's warpgroup MMA (4 warps issue together, accumulators in registers) ----
+// Shared-memory matrix descriptor (cute::GmmaDescriptor), no swizzle ("interleave"):
+// start address, leading / stride byte offsets (all >> 4), layout type 0.
+__device__ __forceinline__ uint64_t wgmma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
     return uint64_t((saddr >> 4) & 0x3fffu) | (uint64_t((lbo_bytes >> 4) & 0x3fffu) << 16)
-        | (uint64_t((sbo_bytes >> 4) & 0x3fffu) << 32) | (uint64_t(1) << 46);
+        | (uint64_t((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor) for kind::tf32, fp32 accumulate.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t M, uint32_t N, bool a_mn_major, bool b_mn_major)
+// orders this thread's register and shared-memory accesses before the wgmma that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// waits until at most N committed wgmma groups of this thread are still in flight
+template<int N> __device__ __forceinline__ void wgmma_wait()
+{ asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+// D[64 x 16] (+)= A[smem, 64 x 8] * B[smem, 8 x 16], kind tf32, both operands K-major, fp32 accumulate.
+// Thread (warp w, lane l) holds d[i] = D[16w + l/4 + 8*((i/2)%2)][8*(i/4) + 2*(l%4) + i%2].
+__device__ __forceinline__ void wgmma_m64n16k8_tf32(float (&d)[8], uint64_t adesc, uint64_t bdesc, bool accumulate)
 {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (uint32_t(a_mn_major) << 15) | (uint32_t(b_mn_major) << 16)
-        | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem], issued by ONE thread for the CTA
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate)
-{
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(uint32_t(accumulate)) : "memory");
-}
-// all MMAs issued so far by this thread arrive on the mbarrier when they have completed
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{ asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory"); }
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp gets lane (base lane + i)
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float (&v)[16])
-{
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    #pragma unroll
-    for(int i = 0;i < 16;++i) v[i] = __uint_as_float(r[i]);
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+                 "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(uint32_t(accumulate)) : "memory");
 }
 
 } // namespace b200mix

@@ -1,4 +1,4 @@
-// effect_kernels.cuh — aux-send wet mix and the convolution effect slot on sm_100a.
+// effect_kernels.cuh — aux-send wet mix and the convolution effect slot on sm_90a.
 //
 //  k_send_mix        MixSamples of every (voice, send) into the slot wet buffers
 //                    (core/voice.cpp:967-980), slot-major and in a fixed order (no atomics)

@@ -1,22 +1,21 @@
-// panmix_tc.cuh — the dense ambisonic pan-mix on the 5th-generation tensor cores.
+// panmix_tc.cuh — the dense ambisonic pan-mix on Hopper's warpgroup tensor cores (wgmma).
 //
 // A device that mixes above first order (config 4a: third-order B-Format output, 16 dry
 // channels) sums every voice into every channel: Dry[c][i] += line_v[i] * gain_v,c — the
 // reference's MixSamples 1->many (core/mixer/mixer_c.cpp:150-186) over all voices is the
 // contraction  Dry[16 x 1024] = G[16 x V] . S[V x 1024], a true dense GEMM with K = voices.
 // Past the gain fade (Counter <= 64 samples, core/voice.cpp:1093) the gains are constants, so
-// samples 128..1023 of every line go through tcgen05.mma:
+// samples 128..1023 of every line go through wgmma.mma_async, one warpgroup per CTA:
 //
-//   D[M = 128 samples][N = 16 channels] (+)= A[M x K = 8 voices] . B[K x N]      (kind::tf32)
+//   D[M = 64 samples][N = 16 channels] += A[M x K = 8 voices] . B[K x N]      (tf32, 14 M tiles)
 //
-//   A = the parked lines.  They lie with the samples (M) contiguous, but kind::tf32 takes its
-//       shared-memory operands K-major only (an MN-major descriptor yields zeros — measured,
-//       tools/ubench/umma_probe.cu), so the lines are transposed on their way into shared memory:
-//       8-row x 16-byte core matrices, (m%8)*16 + (m/8)*SBO + (k/4)*LBO + (k%4)*4, with
-//       LBO = 144 and SBO = 288 bytes so that the transposing scalar stores are conflict-free.
+//   A = the parked lines.  They lie with the samples (M) contiguous, but wgmma takes tf32
+//       shared-memory operands K-major only, so the lines are transposed on their way into
+//       shared memory: 8-row x 16-byte core matrices, (m%8)*16 + (m/8)*SBO + (k/4)*LBO + (k%4)*4,
+//       with LBO = 144 and SBO = 288 bytes so that the transposing scalar stores are conflict-free.
 //   B = geff[entry][channel] (k_send_gains_prepare), K-major
-//   D = fp32 accumulators in TENSOR MEMORY, 7 sample tiles x 16 columns, accumulated over ALL
-//       the voices a CTA owns and read back once (tcgen05.ld) into the CTA's partial row.
+//   D = fp32 accumulators in registers (14 tiles x 8 per thread), accumulated over ALL the
+//       voices a CTA owns, transposed through shared memory into the CTA's partial row.
 //
 // fp32 parity from tf32 tensor cores: both operands are split  x = hi + lo  with hi = x rounded
 // to tf32 and lo = x - hi (exact), and three MMAs accumulate hi.hi + lo.hi + hi.lo; the dropped
@@ -33,14 +32,16 @@
 
 namespace b200mix {
 
-constexpr int kPmTiles = 7;                         // sample tiles 1..7 of 128 (896 samples)
+constexpr int kPmTiles = 7;                         // staged sample tiles 1..7 of 128 (896 samples)
+constexpr int kPmMmaTiles = 2*kPmTiles;             // wgmma M tiles of 64 samples
 constexpr int kPmK = 8;                             // voices per MMA (tf32: 32 bytes of K)
 constexpr int kPmN = 16;                            // channels (padded)
 constexpr int kPmLboA = 144, kPmSboA = 288;         // A core-matrix strides (padded: conflict-free stores)
 constexpr int kPmTileBytes = 16*kPmSboA;            // one A tile: 16 groups of 8 samples x 2 K halves
 constexpr int kPmStageBytes = 2*kPmTiles*kPmTileBytes + 2*kPmN*kPmK*4;     // A hi, A lo, B hi, B lo
 constexpr int kPmStages = 2;
-constexpr uint32_t kPmTmemCols = 128;               // 7 x 16 columns, power of two
+constexpr int kPmOutStride = 7*128 + 4;             // epilogue rows in shared memory (conflict-free stores)
+static_assert(kPmN*kPmOutStride*4 <= kPmStages*kPmStageBytes, "epilogue staging fits the stages");
 
 struct PanMixTcParams {
     const uint32_t *slot_start;     // [2] entry range of the dry bus
@@ -61,12 +62,11 @@ __device__ __forceinline__ void tf32_split(float x, float &hi, float &lo)
     lo = __uint_as_float(__float_as_uint(x - hi) & 0xffffe000u);
 }
 
-// grid = chunks (the entry ranges k_send_mix uses), 128 threads, kPmStages*kPmStageBytes dynamic smem
+// grid = chunks (the entry ranges k_send_mix uses), 128 threads (one warpgroup),
+// kPmStages*kPmStageBytes dynamic smem
 __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
 {
     extern __shared__ __align__(1024) unsigned char pm_smem[];
-    __shared__ uint64_t bar_free[kPmStages];
-    __shared__ uint32_t tmem_slot;
     const uint32_t t = threadIdx.x, warp = t >> 5, lane = t & 31u;
 
     uint32_t e0 = Q.slot_start[0], e1 = Q.slot_start[1];
@@ -78,17 +78,7 @@ __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
     const uint32_t nkb = (e1 - e0 + uint32_t(kPmK) - 1u)/uint32_t(kPmK);
     float *out = Q.partial + size_t(blockIdx.x)*Q.cw*kLine;
 
-    if(warp == 0) tmem_alloc<kPmTmemCols>(&tmem_slot);
-    if(t == 0)
-    {
-        for(int s = 0;s < kPmStages;++s) mbar_init(&bar_free[s], 1u);
-        mbar_fence_init();
-    }
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem = tmem_slot;
-    constexpr uint32_t idesc = umma_idesc_tf32(128u, uint32_t(kPmN), /*A K-major*/false, /*B K-major*/false);
+    float acc[kPmMmaTiles][8];                           // defined by the first K block's MMAs
 
     // this thread's voice of a K block and its sample groups (4 consecutive samples each)
     const uint32_t kk = t & 7u, gl = t >> 3;             // gl in [0,16)
@@ -96,8 +86,7 @@ __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
     {
         const uint32_t st = kb % uint32_t(kPmStages);
         unsigned char *stage = pm_smem + size_t(st)*kPmStageBytes;
-        if(kb >= uint32_t(kPmStages))                    // the MMAs that read this stage are done
-            mbar_wait(&bar_free[st], ((kb / uint32_t(kPmStages)) - 1u) & 1u);
+        // (the MMAs that read this stage, K block kb - kPmStages, were waited for below)
         // ---- A: 8 lines x 896 samples, split, transposed into K-major core matrices
         const uint32_t e = e0 + kb*uint32_t(kPmK) + kk;
         const bool live = e < e1;
@@ -141,54 +130,44 @@ __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
         }
         fence_proxy_async_smem();                        // generic-proxy stores -> tensor core reads
         __syncthreads();
-        if(t == 0)
         {
-            tc_fence_after_sync();
             const uint32_t sa = smem_u32(stage);
             const uint32_t sb = sa + 2u*kPmTiles*kPmTileBytes;
-            const uint64_t bhi = umma_smem_desc(sb, 128u, 256u), blo = umma_smem_desc(sb + kPmN*kPmK*4, 128u, 256u);
+            const uint64_t bhi = wgmma_smem_desc(sb, 128u, 256u), blo = wgmma_smem_desc(sb + kPmN*kPmK*4, 128u, 256u);
+            wgmma_fence();
             #pragma unroll
-            for(int tile = 0;tile < kPmTiles;++tile)
+            for(int q = 0;q < kPmMmaTiles;++q)
             {
-                const uint64_t ahi = umma_smem_desc(sa + uint32_t(tile)*kPmTileBytes, kPmLboA, kPmSboA);
-                const uint64_t alo = umma_smem_desc(sa + uint32_t(kPmTiles + tile)*kPmTileBytes, kPmLboA, kPmSboA);
-                const uint32_t d = tmem + uint32_t(tile)*uint32_t(kPmN);
-                umma_tf32(d, ahi, bhi, idesc, kb != 0u);
-                umma_tf32(d, alo, bhi, idesc, true);
-                umma_tf32(d, ahi, blo, idesc, true);
+                // M tile q = samples 64q..64q+63: the 8-row groups 8(q%2).. of staged tile q/2
+                const uint32_t a = sa + uint32_t(q >> 1)*kPmTileBytes + uint32_t(q & 1)*8u*kPmSboA;
+                const uint64_t ahi = wgmma_smem_desc(a, kPmLboA, kPmSboA);
+                const uint64_t alo = wgmma_smem_desc(a + uint32_t(kPmTiles*kPmTileBytes), kPmLboA, kPmSboA);
+                wgmma_m64n16k8_tf32(acc[q], ahi, bhi, kb != 0u);
+                wgmma_m64n16k8_tf32(acc[q], alo, bhi, true);
+                wgmma_m64n16k8_tf32(acc[q], ahi, blo, true);
             }
-            umma_commit(&bar_free[st]);                  // arrives when these MMAs have completed
+            wgmma_commit();
         }
+        wgmma_wait<kPmStages - 1>();                     // the stage written next iteration is free
     }
-    // ---- all MMAs done: the last commit of every stage in use
-    for(uint32_t s = 0;s < uint32_t(kPmStages);++s)
-    {
-        if(nkb <= s) continue;
-        const uint32_t uses = (nkb - 1u - s)/uint32_t(kPmStages) + 1u;      // commits on this stage
-        mbar_wait(&bar_free[s], (uses - 1u) & 1u);
-    }
-    tc_fence_after_sync();
-    // ---- epilogue: TMEM -> registers -> the CTA's partial row (samples 128..1023)
-    //      warp w reads lanes 32w..32w+31 of every tile = samples 128 + tile*128 + 32w + lane
-    #pragma unroll 1
-    for(int tile = 0;tile < kPmTiles;++tile)
-    {
-        float v[16];
-        if(nkb)
-            tmem_ld_32x16(tmem + ((warp*32u) << 16) + uint32_t(tile)*uint32_t(kPmN), v);
-        else
-        {
-            #pragma unroll
-            for(int c = 0;c < 16;++c) v[c] = 0.0f;
-        }
-        const uint32_t i = 128u + uint32_t(tile)*128u + warp*32u + lane;
-        #pragma unroll
-        for(int c = 0;c < 16;++c)
-            if(uint32_t(c) < Q.cw) out[size_t(c)*kLine + i] = v[c];
-    }
-    tc_fence_before_sync();
+    wgmma_wait<0>();
     __syncthreads();
-    if(warp == 0) tmem_dealloc<kPmTmemCols>(tmem);
+    // ---- epilogue: registers -> shared [channel][sample] -> the CTA's partial row (samples 128..1023)
+    float *so = reinterpret_cast<float*>(pm_smem);
+    #pragma unroll
+    for(int q = 0;q < kPmMmaTiles;++q)
+        #pragma unroll
+        for(int i = 0;i < 8;++i)
+        {
+            const uint32_t m = uint32_t(q)*64u + warp*16u + (lane >> 2) + 8u*((uint32_t(i) >> 1) & 1u);
+            const uint32_t n = uint32_t(i >> 2)*8u + (lane & 3u)*2u + (uint32_t(i) & 1u);
+            so[n*uint32_t(kPmOutStride) + m] = nkb ? acc[q][i] : 0.0f;
+        }
+    __syncthreads();
+    for(uint32_t c = 0;c < Q.cw;++c)
+        for(uint32_t i = t;i < uint32_t(kPmTiles*128/4);i += 128u)
+            reinterpret_cast<float4*>(out + size_t(c)*kLine + 128)[i]
+                = reinterpret_cast<const float4*>(so + c*uint32_t(kPmOutStride))[i];
 }
 
 } // namespace b200mix

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "openal-soft_b200"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "ref: needs the compiled reference under oracle/_ref")
 
 
@@ -28,6 +28,6 @@ def pytest_collection_modifyitems(config, items):
     have_gpu = _has_gpu()
     for item in items:
         if "gpu" in item.keywords and not have_gpu:
-            item.add_marker(pytest.mark.skip(reason="no CUDA device here (runs on the B200 box)"))
+            item.add_marker(pytest.mark.skip(reason="no CUDA device here (runs on an H100)"))
         if "ref" in item.keywords and not have_ref:
             item.add_marker(pytest.mark.skip(reason="oracle/_ref not built"))

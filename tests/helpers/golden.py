@@ -12,9 +12,8 @@ from .mixlib import MixDevice
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "golden")
 
 
-# Fixtures added after the round's GPU minutes were spent (the pitch shifter): their GPU replay lives in
-# tests/test_gpu_zz_pshifter.py, which sorts last, so that under `pytest -x` a first hardware run of
-# new code cannot hide the tests already validated on a B200.  The CPU tests treat them like any other.
+# The pitch shifter's fixtures: their GPU replay lives in tests/test_gpu_zz_pshifter.py, which sorts
+# last, so that under `pytest -x` it cannot hide the other GPU tests.  The CPU tests treat them like any other.
 LATE = ("efx_pshifter_hrtf_v5", "efx_pshifter_down_stereo_v4")
 
 

@@ -4,6 +4,8 @@ of oracle/ref_harness.cpp.  TEST INFRASTRUCTURE ONLY."""
 import ctypes as C
 import os
 import sys
+import tempfile
+
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -103,8 +105,9 @@ def libs(conf_text: str | None = None):
     global _libs
     if _libs is not None:
         return _libs
-    conf_path = os.path.join(REF_DIR, f"alsoft_{os.getpid()}.conf")
-    with open(conf_path, "w") as f:
+    # outside the tree, which may be read-only
+    fd, conf_path = tempfile.mkstemp(prefix="alsoft_", suffix=".conf")
+    with os.fdopen(fd, "w") as f:
         f.write(conf_text or "[general]\n")
     os.environ["ALSOFT_CONF"] = conf_path
     import atexit

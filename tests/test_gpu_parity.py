@@ -756,7 +756,9 @@ def test_efx_effects_vs_oracle_ragged_updates(kind):
     efx_case(kind, *EFX_CASES[kind])
 
 
-def efx_case(kind, typ, setup, change, product=None):
+def efx_case(kind, typ, setup, change, product=None, perturb=None):
+    """The two-slot chain of `typ` through the C ABI, `product` (default: the CUDA library) against
+    the oracle.  `perturb`, if given, changes the send gains the product run uses."""
     rng = np.random.default_rng(300 + typ)
     nv, ir = 12, 64
     desc = synth.hrtf_desc(nv, ir)
@@ -793,7 +795,7 @@ def efx_case(kind, typ, setup, change, product=None):
         return np.concatenate(o, axis=1)
 
     ref = run(mixlib.oracle(), send)
-    out = run(product() if product else mixlib.product(), send)
+    out = run(product() if product else mixlib.product(), perturb(send) if perturb else send)
     # Conditioning: the waveshaper (small-signal gain (1+fc)^3), the high-gain peaking filters and
     # the envelope-driven wah amplify last-bit differences of their INPUT (the send mix sums in a
     # different order on the GPU) by orders of magnitude.  The oracle itself, fed send gains two

@@ -1,4 +1,4 @@
-"""Drop-in scenes added after this round's GPU minutes were spent (tests/test_gpu_dropin.py's
+"""Drop-in scenes of higher-order B-Format beds (tests/test_gpu_dropin.py's
 comparison, libopenal_b200.so + libb200mix.so against the stock reference): second- / third-order
 B-Format beds (AL_SOFT_bformat_hoa) on first-order devices, and beds up to fourth order on
 ALC_BFORMAT3D_SOFT devices of order 2 / 3 (the reference's AmbiRotator turning them).  The CPU half of the same scenes —

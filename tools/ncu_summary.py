@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Summarises an .ncu-rep (one `ncu --set full` capture of k_mix_voices) into the text
-files committed under profiles/: headline metrics, stall mix, and stall samples per
+"""Summarises an .ncu-rep (one `ncu --set full` capture of k_mix_voices) into a text
+file: headline metrics, stall mix, and stall samples per
 barrier-delimited code region.   usage: ncu_summary.py <file.ncu-rep> <out.txt>"""
 import csv
 import io

@@ -1,5 +1,5 @@
 // Standalone check of k_panmix_tc (csrc/panmix_tc.cuh) against a double-precision CPU sum.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++20 -o panmix_tc_test panmix_tc_test.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++20 -o panmix_tc_test panmix_tc_test.cu
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>

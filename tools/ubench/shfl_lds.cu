@@ -1,5 +1,5 @@
 // Microbenchmark: do SHFL.IDX and LDS share one per-SM bandwidth, or do they add?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o shfl_lds shfl_lds.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o shfl_lds shfl_lds.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -34,16 +34,16 @@ __global__ void __launch_bounds__(128) k(float *out, int iters, const int *idx)
 template<int MODE> float run(float *out, const int *idx, int iters)
 {
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    k<MODE><<<148*4, 128>>>(out, 10, idx);
+    k<MODE><<<132*4, 128>>>(out, 10, idx);
     cudaEventRecord(e0);
-    k<MODE><<<148*4, 128>>>(out, iters, idx);
+    k<MODE><<<132*4, 128>>>(out, iters, idx);
     cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1); return ms;
 }
 
 int main()
 {
-    float *out; int *idx; cudaMalloc(&out, 148*4*128*4); cudaMalloc(&idx, 128);
+    float *out; int *idx; cudaMalloc(&out, 132*4*128*4); cudaMalloc(&idx, 128);
     int h[32]; for(int i = 0;i < 32;++i) h[i] = (i*7 + 3) & 31;
     cudaMemcpy(idx, h, 128, cudaMemcpyHostToDevice);
     const int iters = 20000;
