@@ -20,7 +20,8 @@
 // fp32 parity from tf32 tensor cores: both operands are split  x = hi + lo  with hi = x rounded
 // to tf32 and lo = x - hi (exact), and three MMAs accumulate hi.hi + lo.hi + hi.lo; the dropped
 // lo.lo term and lo's own truncation are ~2^-22 relative per product, an order below the parity
-// budget (tests: at-size oracle comparison and ambi3 goldens within 1e-6).
+// budget (tests/test_gpu_panmix.py: this kernel alone against a float64 sum, and the mixer's
+// dry bus against the oracle on the tensor cores and on the SIMT path).
 // Samples 0..127 (the fades) stay with k_send_mix<16>'s first tile; both kernels write disjoint
 // columns of the same per-chunk partial rows, k_reduce_rows sums the chunks in fixed order.
 #pragma once
@@ -86,7 +87,7 @@ __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
     {
         const uint32_t st = kb % uint32_t(kPmStages);
         unsigned char *stage = pm_smem + size_t(st)*kPmStageBytes;
-        // (the MMAs that read this stage, K block kb - kPmStages, were waited for below)
+        // (the MMAs that read this stage, K block kb - kPmStages, were waited for by every warp below)
         // ---- A: 8 lines x 896 samples, split, transposed into K-major core matrices
         const uint32_t e = e0 + kb*uint32_t(kPmK) + kk;
         const bool live = e < e1;
@@ -148,7 +149,8 @@ __global__ void __launch_bounds__(128, 1) k_panmix_tc(const PanMixTcParams Q)
             }
             wgmma_commit();
         }
-        wgmma_wait<kPmStages - 1>();                     // the stage written next iteration is free
+        wgmma_wait<kPmStages - 1>();                     // this warp's share of group kb - 1 is done
+        __syncthreads();    // wait_group covers only this warp's MMAs: all 4 must wait before the stage is rewritten
     }
     wgmma_wait<0>();
     __syncthreads();
