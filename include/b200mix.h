@@ -851,14 +851,16 @@ B200MIX_API int64_t b200mix_get_resampler_table(b200mix_device *dev, uint32_t wh
  * of SURVEY §8(d)'s algorithmic flop count.  < 0 on bad arguments. */
 B200MIX_API int b200mix_resampler_taps(b200mix_device *dev, uint32_t resampler, uint32_t step,
     uint32_t *full);
-/* Kernel timing for roofline reports: when enabled, the voice kernel of every update is
+/* Kernel timing for roofline reports: when enabled, the voice loop of every update (the
+ * resample kernel through the HRIR FIR kernel, with the direct filters between them) is
  * bracketed by CUDA events on the device's stream; b200mix_last_mix_kernel_ms returns the
  * duration of the most recent one (synchronises the stream), <0 if unavailable. */
 B200MIX_API int b200mix_profile(b200mix_device *dev, int enable);
 /* With b200mix_profile(dev, 2) every update also records stage marks; this returns the
- * durations (ms) of the last update's 8 stages: 0 clear, 1 voice kernel, 2 direct filters +
- * deferred voice pass, 3 row reduction, 4 parked dry bus, 5 aux sends, 6 effect slots +
- * slot output mix, 7 post-process.  Returns the stage count, <0 if unavailable. */
+ * durations (ms) of the last update's 8 stages: 0 clear, 1 resample kernel, 2 direct filters
+ * + deferred dry pass + HRIR FIR kernel, 3 row reduction, 4 parked dry bus, 5 aux sends,
+ * 6 effect slots + slot output mix, 7 post-process.  Returns the stage count, <0 if
+ * unavailable. */
 B200MIX_API int b200mix_last_stage_ms(b200mix_device *dev, float *ms, uint32_t count);
 B200MIX_API float b200mix_last_mix_kernel_ms(b200mix_device *dev);
 /* Number of CUDA kernels this device has launched so far. */

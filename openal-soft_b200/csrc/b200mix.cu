@@ -223,6 +223,8 @@ struct b200mix_device {
     int mix_variant{0}; int mix_groups{2}; int mix_gs{64}; int mix_cdr{0};
     uint32_t reverb_seq{0};          // update counter of k_reverb_process' early/late hand-off (24 bits used)
     size_t mix_smem{0}; int mix_blocks_per_sm{1};
+    uint32_t *d_claim{nullptr};      // voice claim counters of the parking k_mix_voices
+    int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
 };
 
 namespace {
@@ -242,26 +244,30 @@ int dev_alloc(b200mix_device *d, T *&p, size_t count, bool zero = true)
 
 using MixKernel = void(*)(const MixParams);
 
-struct Variant { MixKernel fn; int gs, groups, cdr; size_t smem; bool hrtf; };
+struct Variant { MixKernel fn; int gs, groups, cdr; size_t smem; };
 
-template<int GS, int GROUPS, bool HRTF, int CDR, int OPT, int FP>
+template<int GS, int GROUPS, int CDR>
 Variant make_variant()
 {
-    return Variant{k_mix_voices<GS, GROUPS, HRTF, CDR, OPT, FP>, GS, GROUPS, CDR,
-        sizeof(GroupSmem<GS, OPT, FP>)*GROUPS, HRTF};
+    return Variant{k_mix_voices<GS, GROUPS, CDR>, GS, GROUPS, CDR, sizeof(GroupSmem<CDR>)*GROUPS};
 }
 
-// 0: HRTF ir<=64, 1: HRTF ir<=128, 2: dry <=4 channels in registers,
-// 3: wider dry mixes: resample + park, the dry bus is summed by k_send_mix
+// 0: non-HRTF devices with <= 4 dry channels: the dry bus is mixed in registers,
+// 1: HRTF devices and wider dry mixes: resample + park; k_hrtf_fir mixes the HRTF voices,
+//    k_send_mix sums the dry bus
 Variant get_variant(int idx)
 {
-    switch(idx)
-    {
-    case 0: return make_variant<64, 2, true, 0, 17, 64>();
-    case 1: return make_variant<64, 2, true, 0, 19, 128>();
-    case 2: return make_variant<64, 2, false, 4, 1, 8>();
-    default: return make_variant<64, 2, false, 0, 1, 8>();
-    }
+    return idx == 0 ? make_variant<64, 2, 4>() : make_variant<64, 2, 0>();
+}
+
+// HRIR FIR kernel of an HRTF device: 17 outputs per thread / 64 front pad for ir <= 64,
+// 19 / 128 for ir <= 128
+struct FirVariant { MixKernel fn; size_t smem; };
+FirVariant get_fir(uint32_t ir_size)
+{
+    if(ir_size <= 64u)
+        return FirVariant{k_hrtf_fir<17, 64>, sizeof(FirSmem<kFirGS, 17, 64>)*kFirGroups};
+    return FirVariant{k_hrtf_fir<19, 128>, sizeof(FirSmem<kFirGS, 19, 128>)*kFirGroups};
 }
 
 constexpr uint32_t kDryChunksMax = 128;
@@ -422,13 +428,29 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
 
         // launch variant
         const bool hrtfDev = dd.ir_size > 0;
-        d->mix_variant = hrtfDev ? (dd.ir_size <= 64 ? 0 : 1) : (dd.dry_channels <= 4 ? 2 : 3);
+        d->mix_variant = (!hrtfDev && dd.dry_channels <= 4) ? 0 : 1;
         const Variant var = get_variant(d->mix_variant);
         d->mix_gs = var.gs; d->mix_groups = var.groups; d->mix_cdr = var.cdr; d->mix_smem = var.smem;
         CUDA_TRY(d, cudaFuncSetAttribute(var.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(var.smem)));
         int perSm = 0;
         CUDA_TRY(d, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, var.fn, var.gs*var.groups, var.smem));
         d->mix_blocks_per_sm = std::max(perSm, 1);
+        if(var.cdr == 0)
+        {
+            // the parking variant writes every mixed voice's line and state bits
+            if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
+            if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
+            if(int rc = dev_alloc(d, d->d_claim, 2)) return rc;
+        }
+        if(hrtfDev)
+        {
+            const FirVariant fir = get_fir(dd.ir_size);
+            CUDA_TRY(d, cudaFuncSetAttribute(fir.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(fir.smem)));
+            CUDA_TRY(d, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, fir.fn, kFirGS*kFirGroups, fir.smem));
+            // the FIR grid sets the partial rows, hence the summation order: it is fixed at
+            // kFirCtasPerSm per SM (the launch bounds), not at whatever more might fit
+            d->fir_blocks_per_sm = std::max(std::min(perSm, kFirCtasPerSm), 1);
+        }
 
         d->dry_alloc_ch = std::max<uint32_t>(std::max(dd.dry_channels, 1u), uint32_t(var.cdr));
         if(int rc = dev_alloc(d, d->d_dry, size_t(d->dry_alloc_ch)*kLine)) return rc;
@@ -451,10 +473,11 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         }
         if(dd.max_slots && dd.wet_channels)
             if(int rc = dev_alloc(d, d->d_wet, size_t(dd.max_slots)*dd.wet_channels*kLine)) return rc;
-        const size_t maxRows = size_t(d->num_sms)*d->mix_blocks_per_sm;
-        d->partial_floats = maxRows*(hrtfDev ? 2*kAccumLen : 0) + maxRows*size_t(var.cdr)*kLine;
-        // two regions: the main pass and the deferred pass of voices with direct filters
-        if(int rc = dev_alloc(d, d->d_partial, std::max<size_t>(2*d->partial_floats, 4))) return rc;
+        // partial rows: the FIR's HrtfAccumData rows (HRTF devices), or the register dry bus'
+        // rows in two regions, the main pass and the deferred pass of voices with direct filters
+        d->partial_floats = hrtfDev ? size_t(d->num_sms)*d->fir_blocks_per_sm*(2*kAccumLen)
+            : size_t(d->num_sms)*d->mix_blocks_per_sm*size_t(var.cdr)*kLine;
+        if(int rc = dev_alloc(d, d->d_partial, std::max<size_t>((hrtfDev ? 1 : 2)*d->partial_floats, 4))) return rc;
         if(int rc = dev_alloc(d, d->d_accum_sum, 2*kAccumLen)) return rc;
         if(int rc = dev_alloc(d, d->d_carry[0], 2*kHrirLen)) return rc;
         if(int rc = dev_alloc(d, d->d_carry[1], 2*kHrirLen)) return rc;
@@ -465,8 +488,10 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
             d->h_slots.assign(dd.max_slots, SlotRec{});
             d->slot_allocs.assign(dd.max_slots, {});
             if(int rc = dev_alloc(d, d->d_slots, dd.max_slots)) return rc;
-            if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
-            if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
+            if(!d->d_xscratch)
+                if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
+            if(!d->d_sendinfo)
+                if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
             if(int rc = dev_alloc(d, d->d_send_geff, size_t(dd.max_voices)*dd.num_sends*dd.wet_channels)) return rc;
             if(int rc = dev_alloc(d, d->d_send_gramp, size_t(dd.max_voices)*dd.num_sends*dd.wet_channels)) return rc;
             d->h_send_slot.assign(size_t(dd.max_voices)*B200MIX_MAX_SENDS, B200MIX_NO_SLOT);
@@ -524,7 +549,7 @@ void b200mix_destroy(b200mix_device *d)
     cudaFree(d->d_uhj_state); cudaFree(d->d_uhj_scratch);
     cudaFree(d->d_uhj_fir_state); cudaFree(d->d_uhj_fir_coef); cudaFree(d->d_bs2b); cudaFree(d->d_stab_state);
     for(auto &v : d->slot_allocs) for(void *p : v) cudaFree(p);
-    cudaFree(d->d_slots); cudaFree(d->d_xscratch); cudaFree(d->d_sendinfo);
+    cudaFree(d->d_slots); cudaFree(d->d_xscratch); cudaFree(d->d_sendinfo); cudaFree(d->d_claim);
     cudaFree(d->d_filt); cudaFree(d->d_fupd); cudaFree(d->d_fscratch);
     cudaFree(d->d_dline); cudaFree(d->d_order2); cudaFree(d->d_qhdr); cudaFree(d->d_queue);
     cudaFree(d->d_outbuf); if(d->h_outbuf) cudaFreeHost(d->h_outbuf);
@@ -1730,10 +1755,10 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         d->order2_dirty = false;
     }
     const Variant var = get_variant(d->mix_variant);
+    const bool hrtfDev = dd.ir_size > 0;
     const uint32_t nv = std::max(d->voice_hi, 1u);
     const uint32_t maxBlocks = uint32_t(d->num_sms*d->mix_blocks_per_sm);
     const uint32_t blocks = std::max(1u, std::min(maxBlocks, (d->num_order + var.groups - 1)/var.groups));
-    const size_t rows = size_t(blocks);        // one partial row per CTA
 
     MixParams P{};
     P.voices = d->d_voices; P.buffers = d->d_buffers;
@@ -1752,10 +1777,12 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     P.filt = d->d_filt; P.filt_paths = 1u + dd.num_sends;
     P.qhdr = d->d_qhdr; P.queue = d->d_queue;
     P.gather_only = d->mix_gather_only ? 1u : 0u;
+    P.claim = d->d_claim;
+    P.dline = d->d_dline;
+    // the voice loop: resample (and park) -> direct filters -> deferred dry pass or HRIR FIR
     stage_mark(d, 1);
     if(d->profile) cudaEventRecord(d->ev_mix0, d->stream);
     var.fn<<<blocks, var.gs*var.groups, var.smem, d->stream>>>(P);
-    if(d->profile) { cudaEventRecord(d->ev_mix1, d->stream); d->ev_valid = true; }
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
 
@@ -1770,42 +1797,49 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         FP.xscratch = d->d_xscratch; FP.dline = d->d_dline; FP.frames = frames;
         k_filters<<<(d->num_order2 + 31u)/32u, 32, 0, d->stream>>>(FP);
         ++d->launches;
-        const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (d->num_order2 + var.groups - 1)/var.groups));
-        rows2 = blocks2;
-        MixParams P2 = P;
-        P2.pass = 1u; P2.dline = d->d_dline;
-        P2.order = d->d_order2; P2.num_order = d->num_order2;
-        P2.partial = d->d_partial + d->partial_floats;
-        P2.results = nullptr;
-        var.fn<<<blocks2, var.gs*var.groups, var.smem, d->stream>>>(P2);
+        if(var.cdr > 0)
+        {
+            const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (d->num_order2 + var.groups - 1)/var.groups));
+            rows2 = blocks2;
+            MixParams P2 = P;
+            P2.pass = 1u;
+            P2.order = d->d_order2; P2.num_order = d->num_order2;
+            P2.partial = d->d_partial + d->partial_floats;
+            P2.results = nullptr;
+            var.fn<<<blocks2, var.gs*var.groups, var.smem, d->stream>>>(P2);
+            ++d->launches;
+        }
+        CUDA_TRY(d, cudaGetLastError());
+    }
+    uint32_t firBlocks = 0;
+    if(hrtfDev)
+    {
+        const FirVariant fir = get_fir(dd.ir_size);
+        firBlocks = std::max(1u, std::min(uint32_t(d->num_sms*d->fir_blocks_per_sm),
+            (d->num_order + kFirGroups - 1)/kFirGroups));
+        fir.fn<<<firBlocks, kFirGS*kFirGroups, fir.smem, d->stream>>>(P);
         ++d->launches;
         CUDA_TRY(d, cudaGetLastError());
     }
+    if(d->profile) { cudaEventRecord(d->ev_mix1, d->stream); d->ev_valid = true; }
 
     stage_mark(d, 3);
-    if(var.hrtf)
+    if(hrtfDev)
     {
         const uint32_t len = 2*kAccumLen;
-        k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial, uint32_t(rows), len,
+        k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial, firBlocks, len,
             d->d_accum_sum, 0);
         ++d->launches;
-        if(rows2)
-        {
-            k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial + d->partial_floats,
-                uint32_t(rows2), len, d->d_accum_sum, 1);
-            ++d->launches;
-        }
     }
     if(var.cdr > 0)
     {
         const uint32_t len = uint32_t(var.cdr)*kLine;
-        const float *pd = d->d_partial + (var.hrtf ? rows*(2*kAccumLen) : 0);
-        k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(pd, uint32_t(rows), len, d->d_dry, 1);
+        k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial, blocks, len, d->d_dry, 1);
         ++d->launches;
         if(rows2)
         {
-            const float *pd2 = d->d_partial + d->partial_floats + (var.hrtf ? rows2*(2*kAccumLen) : 0);
-            k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(pd2, uint32_t(rows2), len, d->d_dry, 1);
+            k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial + d->partial_floats,
+                uint32_t(rows2), len, d->d_dry, 1);
             ++d->launches;
         }
     }
