@@ -196,7 +196,6 @@ struct b200mix_device {
     cudaEvent_t src_done{nullptr}; bool src_busy{false};
     bool dev_filters{false};                 // filter activity is decided on the device: order2 = order
     bool panmix_tc{false};                   // wide dry buses: pan-mix past the fades on the tensor cores
-    bool mix_gather_only{false};             // B200MIX_MIX_GATHER=1: no TMA staging in k_mix_voices (A/B runs)
 
     // voice-sharded device set (b200mix_shard_*): transport 0 none, 1 peer stores, 2 NCCL
     struct Shard {
@@ -219,10 +218,10 @@ struct b200mix_device {
 
     uint32_t ir_pad{0};
     uint32_t voice_hi{0};          // 1 + highest voice index ever configured
-    // launch geometry (resolved at create)
-    int mix_variant{0}; int mix_groups{2}; int mix_gs{64}; int mix_cdr{0};
+    // resample kernel (resolved at create): k_mix_voices<kMixGS, kMixGroups, mix_cdr>
+    void (*mix_fn)(const MixParams){nullptr};
+    size_t mix_smem{0}; int mix_cdr{0}; int mix_blocks_per_sm{1};
     uint32_t reverb_seq{0};          // update counter of k_reverb_process' early/late hand-off (24 bits used)
-    size_t mix_smem{0}; int mix_blocks_per_sm{1};
     uint32_t *d_claim{nullptr};      // voice claim counters of the parking k_mix_voices
     int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
 };
@@ -243,22 +242,6 @@ int dev_alloc(b200mix_device *d, T *&p, size_t count, bool zero = true)
 }
 
 using MixKernel = void(*)(const MixParams);
-
-struct Variant { MixKernel fn; int gs, groups, cdr; size_t smem; };
-
-template<int GS, int GROUPS, int CDR>
-Variant make_variant()
-{
-    return Variant{k_mix_voices<GS, GROUPS, CDR>, GS, GROUPS, CDR, sizeof(GroupSmem<CDR>)*GROUPS};
-}
-
-// 0: non-HRTF devices with <= 4 dry channels: the dry bus is mixed in registers,
-// 1: HRTF devices and wider dry mixes: resample + park; k_hrtf_fir mixes the HRTF voices,
-//    k_send_mix sums the dry bus
-Variant get_variant(int idx)
-{
-    return idx == 0 ? make_variant<64, 2, 4>() : make_variant<64, 2, 0>();
-}
 
 // HRIR FIR kernel of an HRTF device: 17 outputs per thread / 64 front pad for ir <= 64,
 // 19 / 128 for ir <= 128
@@ -362,7 +345,6 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
     auto *d = new(std::nothrow) b200mix_device{};
     if(!d) { g_create_error = "out of host memory"; return B200MIX_ERR_NOMEM; }
     d->desc = *desc;
-    if(const char *g = std::getenv("B200MIX_MIX_GATHER")) d->mix_gather_only = g[0] == '1';
     auto fail = [&](int code) { g_create_error = d->error; b200mix_destroy(d); return code; };
 
     int count = 0;
@@ -426,16 +408,28 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         d->h_cost.assign(dd.max_voices, 0);
         d->h_hrtf.assign(dd.max_voices, 0);
 
-        // launch variant
+        // resample kernel: non-HRTF devices with <= 4 dry channels mix the dry bus in registers;
+        // HRTF devices and wider dry mixes resample + park (k_hrtf_fir mixes the HRTF voices,
+        // k_send_mix sums the dry bus)
         const bool hrtfDev = dd.ir_size > 0;
-        d->mix_variant = (!hrtfDev && dd.dry_channels <= 4) ? 0 : 1;
-        const Variant var = get_variant(d->mix_variant);
-        d->mix_gs = var.gs; d->mix_groups = var.groups; d->mix_cdr = var.cdr; d->mix_smem = var.smem;
-        CUDA_TRY(d, cudaFuncSetAttribute(var.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(var.smem)));
+        if(!hrtfDev && dd.dry_channels <= 4)
+        {
+            d->mix_cdr = 4;
+            d->mix_fn = k_mix_voices<kMixGS, kMixGroups, 4>;
+            d->mix_smem = sizeof(GroupSmem<4>)*kMixGroups;
+        }
+        else
+        {
+            d->mix_cdr = 0;
+            d->mix_fn = k_mix_voices<kMixGS, kMixGroups, 0>;
+            d->mix_smem = sizeof(GroupSmem<0>)*kMixGroups;
+        }
+        CUDA_TRY(d, cudaFuncSetAttribute(d->mix_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, int(d->mix_smem)));
         int perSm = 0;
-        CUDA_TRY(d, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, var.fn, var.gs*var.groups, var.smem));
+        CUDA_TRY(d, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, d->mix_fn, kMixGS*kMixGroups,
+            d->mix_smem));
         d->mix_blocks_per_sm = std::max(perSm, 1);
-        if(var.cdr == 0)
+        if(d->mix_cdr == 0)
         {
             // the parking variant writes every mixed voice's line and state bits
             if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
@@ -452,7 +446,7 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
             d->fir_blocks_per_sm = std::max(std::min(perSm, kFirCtasPerSm), 1);
         }
 
-        d->dry_alloc_ch = std::max<uint32_t>(std::max(dd.dry_channels, 1u), uint32_t(var.cdr));
+        d->dry_alloc_ch = std::max<uint32_t>(std::max(dd.dry_channels, 1u), uint32_t(d->mix_cdr));
         if(int rc = dev_alloc(d, d->d_dry, size_t(d->dry_alloc_ch)*kLine)) return rc;
         // RealOut and the voice results share one block (and one pinned mirror): a render that
         // returns both needs ONE device-to-host copy
@@ -474,9 +468,9 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         if(dd.max_slots && dd.wet_channels)
             if(int rc = dev_alloc(d, d->d_wet, size_t(dd.max_slots)*dd.wet_channels*kLine)) return rc;
         // partial rows: the FIR's HrtfAccumData rows (HRTF devices), or the register dry bus'
-        // rows in two regions, the main pass and the deferred pass of voices with direct filters
+        // rows in two regions, k_mix_voices' and k_mix_deferred's (voices with direct filters)
         d->partial_floats = hrtfDev ? size_t(d->num_sms)*d->fir_blocks_per_sm*(2*kAccumLen)
-            : size_t(d->num_sms)*d->mix_blocks_per_sm*size_t(var.cdr)*kLine;
+            : size_t(d->num_sms)*d->mix_blocks_per_sm*size_t(d->mix_cdr)*kLine;
         if(int rc = dev_alloc(d, d->d_partial, std::max<size_t>((hrtfDev ? 1 : 2)*d->partial_floats, 4))) return rc;
         if(int rc = dev_alloc(d, d->d_accum_sum, 2*kAccumLen)) return rc;
         if(int rc = dev_alloc(d, d->d_carry[0], 2*kHrirLen)) return rc;
@@ -1692,6 +1686,52 @@ int b200mix_voices_filters(b200mix_device *d, uint32_t n, const b200mix_voice_fi
     return B200MIX_OK;
 }
 
+// One bus mix of parked lines, the parked dry bus (one pseudo slot) or the aux sends (`slots`
+// slots): the entries' gain ramps -> k_send_mix in M.chunks entry chunks, with samples
+// 128..1023 on the tensor cores when `tc` -> the chunks' partial rows summed into M.wet ->
+// the Current gains advanced.
+static int run_bus_mix(b200mix_device *d, const SendMixParams &M, uint32_t num_entries, uint32_t slots,
+    bool tc)
+{
+    const uint32_t chunks = M.chunks;
+    if(num_entries)
+    {
+        const uint32_t tot = num_entries*M.cw;
+        k_send_gains_prepare<<<(tot + 127)/128, 128, 0, d->stream>>>(M, num_entries);
+        ++d->launches;
+    }
+    const uint32_t tiles = tc ? 1u : (chunks > 1u ? uint32_t(kLine/128) : (M.frames + 127u)/128u);
+    if(M.cw > 4u) k_send_mix<16><<<dim3(slots, tiles, chunks), 256, 0, d->stream>>>(M);
+    else k_send_mix<4><<<dim3(slots, tiles, chunks), 256, 0, d->stream>>>(M);
+    ++d->launches;
+    if(tc)
+    {
+        // dline stays null until a direct filter is set: no sendinfo lookups per entry before then
+        PanMixTcParams TQ{M.slot_start, M.entries, M.sendinfo, M.xscratch, d->d_dline, M.geff, M.cw, chunks,
+            M.partial};
+        k_panmix_tc<<<chunks, 128, kPmStages*kPmStageBytes + 1024, d->stream>>>(TQ);
+        ++d->launches;
+    }
+    if(chunks > 1u)
+    {
+        const uint32_t len = slots*M.cw*kLine;
+        if(chunks <= 16u)
+            k_reduce_few<<<(len/4 + 255)/256, 256, 0, d->stream>>>(M.partial, chunks, len, M.wet, 1);
+        else
+            k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(
+                M.partial, chunks, len, M.wet, 1);
+        ++d->launches;
+    }
+    if(num_entries)
+    {
+        const uint32_t tot = num_entries*M.cw;
+        k_send_gains_update<<<(tot + 127)/128, 128, 0, d->stream>>>(M, num_entries);
+        ++d->launches;
+    }
+    CUDA_TRY(d, cudaGetLastError());
+    return B200MIX_OK;
+}
+
 static inline void stage_mark(b200mix_device *d, int i)
 { if(d->profile_level >= 2) cudaEventRecord(d->ev_stage[i], d->stream); }
 
@@ -1743,7 +1783,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     {
         d->h_order2.clear();
         // with the GPU parameter stage the host does not know which direct filters are active:
-        // the second pass then looks at every voice's kSiDeferred bit
+        // k_filters and k_mix_deferred then look at every voice's kSiDeferred bit
         for(uint32_t v : d->h_order) if(d->dev_filters || d->h_dfilt[v]) d->h_order2.push_back(v);
         d->num_order2 = uint32_t(d->h_order2.size());
         if(d->num_order2)
@@ -1754,35 +1794,31 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         }
         d->order2_dirty = false;
     }
-    const Variant var = get_variant(d->mix_variant);
     const bool hrtfDev = dd.ir_size > 0;
     const uint32_t nv = std::max(d->voice_hi, 1u);
     const uint32_t maxBlocks = uint32_t(d->num_sms*d->mix_blocks_per_sm);
-    const uint32_t blocks = std::max(1u, std::min(maxBlocks, (d->num_order + var.groups - 1)/var.groups));
+    const uint32_t blocks = std::max(1u, std::min(maxBlocks, (d->num_order + kMixGroups - 1)/kMixGroups));
 
     MixParams P{};
     P.voices = d->d_voices; P.buffers = d->d_buffers;
     P.hrtf_tgt = d->d_hrtf_tgt; P.hrtf_old = d->d_hrtf_old;
     P.dry_cur = d->d_dry_cur; P.dry_tgt = d->d_dry_tgt;
-    P.send_cur = d->d_send_cur; P.send_tgt = d->d_send_tgt;
-    P.dry = d->d_dry; P.wet = d->d_wet; P.partial = d->d_partial;
+    P.partial = d->d_partial;
     P.results = want_results ? d->d_results : nullptr;
     for(int i = 0;i < 3;++i) P.bsinc_tab[i] = d->d_bsinc[i];
     for(int i = 0;i < 2;++i) P.cubic_tab[i] = d->d_cubic[i];
-    P.max_voices = nv; P.frames = frames; P.ir = dd.ir_size; P.ir_pad = d->ir_pad;
-    P.cd = dd.dry_channels; P.cw = dd.wet_channels; P.num_sends = dd.num_sends;
-    P.max_buffers = dd.max_buffers;
+    P.max_voices = nv; P.frames = frames; P.ir_pad = d->ir_pad;
+    P.cd = dd.dry_channels; P.num_sends = dd.num_sends;
     P.order = d->d_order; P.num_order = d->num_order;
     P.xscratch = d->d_xscratch; P.sendinfo = d->d_sendinfo;
     P.filt = d->d_filt; P.filt_paths = 1u + dd.num_sends;
     P.qhdr = d->d_qhdr; P.queue = d->d_queue;
-    P.gather_only = d->mix_gather_only ? 1u : 0u;
     P.claim = d->d_claim;
     P.dline = d->d_dline;
     // the voice loop: resample (and park) -> direct filters -> deferred dry pass or HRIR FIR
     stage_mark(d, 1);
     if(d->profile) cudaEventRecord(d->ev_mix0, d->stream);
-    var.fn<<<blocks, var.gs*var.groups, var.smem, d->stream>>>(P);
+    d->mix_fn<<<blocks, kMixGS*kMixGroups, d->mix_smem, d->stream>>>(P);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
 
@@ -1797,16 +1833,19 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         FP.xscratch = d->d_xscratch; FP.dline = d->d_dline; FP.frames = frames;
         k_filters<<<(d->num_order2 + 31u)/32u, 32, 0, d->stream>>>(FP);
         ++d->launches;
-        if(var.cdr > 0)
+        if(d->mix_cdr > 0)
         {
-            const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (d->num_order2 + var.groups - 1)/var.groups));
+            // The grid is the number of partial rows, so it fixes the order in which the
+            // deferred voices' sums are added: it follows the resample kernel's occupancy, as
+            // the main pass's does, not this kernel's own.
+            const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (d->num_order2 + kMixGroups - 1)/kMixGroups));
             rows2 = blocks2;
             MixParams P2 = P;
-            P2.pass = 1u;
             P2.order = d->d_order2; P2.num_order = d->num_order2;
             P2.partial = d->d_partial + d->partial_floats;
             P2.results = nullptr;
-            var.fn<<<blocks2, var.gs*var.groups, var.smem, d->stream>>>(P2);
+            k_mix_deferred<kMixGS, kMixGroups, 4><<<blocks2, kMixGS*kMixGroups,
+                sizeof(DeferredSmem<kMixGroups, 4>), d->stream>>>(P2);
             ++d->launches;
         }
         CUDA_TRY(d, cudaGetLastError());
@@ -1831,9 +1870,9 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             d->d_accum_sum, 0);
         ++d->launches;
     }
-    if(var.cdr > 0)
+    if(d->mix_cdr > 0)
     {
-        const uint32_t len = uint32_t(var.cdr)*kLine;
+        const uint32_t len = uint32_t(d->mix_cdr)*kLine;
         k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial, blocks, len, d->d_dry, 1);
         ++d->launches;
         if(rows2)
@@ -1847,7 +1886,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
 
     stage_mark(d, 4);
     // ---- parked dry bus: non-HRTF voices of a variant without register accumulators ----
-    if(var.cdr == 0 && d->d_dry_entries)
+    if(d->mix_cdr == 0 && d->d_dry_entries)
     {
         if(d->dry_entries_dirty)
         {
@@ -1874,41 +1913,12 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             // (fading) tile's serial work per warp short
             const uint32_t chunks = std::max(1u, std::min(kDryChunksMax, (d->num_dry_entries + 63u)/64u));
             DM.chunks = chunks; DM.partial = d->d_dry_partial; DM.geff = d->d_dry_geff; DM.gramp = d->d_dry_gramp;
-            {
-                const uint32_t tot = d->num_dry_entries*dd.dry_channels;
-                k_send_gains_prepare<<<(tot + 127)/128, 128, 0, d->stream>>>(DM, d->num_dry_entries);
-                ++d->launches;
-            }
             // Above 4 dry channels (third-order output) a full update's pan-mix past the gain fades
             // is a dense GEMM over the voices: samples 128..1023 go to the tensor cores
             // (k_panmix_tc), k_send_mix keeps the first tile with the fades
             const bool tc = d->panmix_tc && dd.dry_channels > 4u && dd.dry_channels <= uint32_t(kPmN)
                 && frames == uint32_t(kLine) && chunks > 1u;
-            const uint32_t tiles = tc ? 1u : (chunks > 1u ? uint32_t(kLine/128) : (frames + 127u)/128u);
-            if(dd.dry_channels > 4u) k_send_mix<16><<<dim3(1, tiles, chunks), 256, 0, d->stream>>>(DM);
-            else k_send_mix<4><<<dim3(1, tiles, chunks), 256, 0, d->stream>>>(DM);
-            ++d->launches;
-            if(tc)
-            {
-                PanMixTcParams TQ{d->d_dry_slot_start, d->d_dry_entries, d->d_sendinfo, d->d_xscratch,
-                    d->d_dline, d->d_dry_geff, dd.dry_channels, chunks, d->d_dry_partial};
-                k_panmix_tc<<<chunks, 128, kPmStages*kPmStageBytes + 1024, d->stream>>>(TQ);
-                ++d->launches;
-            }
-            if(chunks > 1u)
-            {
-                const uint32_t len = dd.dry_channels*kLine;
-                if(chunks <= 16u)
-                    k_reduce_few<<<(len/4 + 255)/256, 256, 0, d->stream>>>(d->d_dry_partial, chunks, len, d->d_dry, 1);
-                else
-                k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(
-                    d->d_dry_partial, chunks, len, d->d_dry, 1);
-                ++d->launches;
-            }
-            const uint32_t tot = d->num_dry_entries*dd.dry_channels;
-            k_send_gains_update<<<(tot + 127)/128, 128, 0, d->stream>>>(DM, d->num_dry_entries);
-            ++d->launches;
-            CUDA_TRY(d, cudaGetLastError());
+            if(int rc = run_bus_mix(d, DM, d->num_dry_entries, 1u, tc)) return rc;
         }
     }
 
@@ -1946,7 +1956,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         SM.slot_start = d->d_slot_start; SM.entries = d->d_entries; SM.sendinfo = d->d_sendinfo;
         SM.xscratch = d->d_xscratch; SM.send_cur = d->d_send_cur; SM.send_tgt = d->d_send_tgt;
         SM.wet = d->d_wet; SM.frames = frames; SM.cw = dd.wet_channels; SM.num_sends = dd.num_sends;
-        SM.valid_bit = kSiSend; SM.chunks = 1;
+        SM.valid_bit = kSiSend;
         if(d->d_filt && d->num_entries)
         {
             if(d->fscratch_rows < d->num_entries)
@@ -1967,46 +1977,18 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             ++d->launches;
         }
         SM.geff = d->d_send_geff; SM.gramp = d->d_send_gramp;
-        if(d->num_entries)
+        // a CTA's 8 warps share its entries evenly: chunks of 128 entries per slot
+        const uint32_t chunks = std::max(1u, std::min(16u, (d->max_slot_entries + 127u)/128u));
+        if(chunks > 1u && d->send_partial_chunks < chunks)
         {
-            const uint32_t tot = d->num_entries*dd.wet_channels;
-            k_send_gains_prepare<<<(tot + 127)/128, 128, 0, d->stream>>>(SM, d->num_entries);
-            ++d->launches;
+            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            cudaFree(d->d_send_partial); d->d_send_partial = nullptr; d->send_partial_chunks = 0;
+            CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_send_partial),
+                size_t(chunks)*dd.max_slots*dd.wet_channels*kLine*sizeof(float)));
+            d->send_partial_chunks = chunks;
         }
-        {
-            // a CTA's 8 warps share its entries evenly: chunks of 128 entries per slot
-            const uint32_t chunks = std::max(1u, std::min(16u, (d->max_slot_entries + 127u)/128u));
-            if(chunks > 1u && d->send_partial_chunks < chunks)
-            {
-                CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-                cudaFree(d->d_send_partial); d->d_send_partial = nullptr; d->send_partial_chunks = 0;
-                CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_send_partial),
-                    size_t(chunks)*dd.max_slots*dd.wet_channels*kLine*sizeof(float)));
-                d->send_partial_chunks = chunks;
-            }
-            SM.chunks = chunks; SM.partial = d->d_send_partial;
-            const uint32_t tiles = chunks > 1u ? uint32_t(kLine/128) : (frames + 127u)/128u;
-            if(dd.wet_channels > 4u) k_send_mix<16><<<dim3(dd.max_slots, tiles, chunks), 256, 0, d->stream>>>(SM);
-            else k_send_mix<4><<<dim3(dd.max_slots, tiles, chunks), 256, 0, d->stream>>>(SM);
-            ++d->launches;
-            if(chunks > 1u)
-            {
-                const uint32_t len = dd.max_slots*dd.wet_channels*kLine;
-                if(chunks <= 16u)
-                    k_reduce_few<<<(len/4 + 255)/256, 256, 0, d->stream>>>(d->d_send_partial, chunks, len, d->d_wet, 1);
-                else
-                k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(
-                    d->d_send_partial, chunks, len, d->d_wet, 1);
-                ++d->launches;
-            }
-        }
-        if(d->num_entries)
-        {
-            const uint32_t tot = d->num_entries*dd.wet_channels;
-            k_send_gains_update<<<(tot + 127)/128, 128, 0, d->stream>>>(SM, d->num_entries);
-            ++d->launches;
-        }
-        CUDA_TRY(d, cudaGetLastError());
+        SM.chunks = chunks; SM.partial = d->d_send_partial;
+        if(int rc = run_bus_mix(d, SM, d->num_entries, dd.max_slots, false)) return rc;
     }
     return B200MIX_OK;
 }

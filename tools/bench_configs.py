@@ -60,6 +60,8 @@ def main():
     ap.add_argument("--transport", default="p2p", choices=["p2p", "nccl"])
     ap.add_argument("--steps", type=int, default=16)
     ap.add_argument("--warmup", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed update's RealOut block as DIR/real_out_<config>.npy (float32)")
     args = ap.parse_args()
     import torch
     import torch.distributed as dist
@@ -226,6 +228,13 @@ def main():
         st = np.zeros(8, dtype=np.float32)
         if lib.b200mix_last_stage_ms(h, st.ctypes.data, 8) == 8:
             stages.append(st)
+    if args.dump_outputs and rank == 0:
+        class _Block:
+            __cuda_array_interface__ = {"shape": (desc.real_channels, 1024), "typestr": "<f4",
+                                        "data": (out.value, False), "strides": None, "version": 2}
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"real_out_{args.config}.npy"),
+                torch.as_tensor(_Block(), device="cuda").cpu().numpy())
     t = torch.tensor([float(np.mean(ms))], device="cuda")
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
