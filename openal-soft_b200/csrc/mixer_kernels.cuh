@@ -287,22 +287,40 @@ __device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c)
 
 // One FIR pass for BOTH ears: acc[r].{x,y} += sum_j c[j].{x,y} * in[FP + t0 + r - j].{x,y}
 // (gather form of MixHrtfBase's scatter, hrtfbase.h:28-40).  Taps go in blocks of JB with a
-// register window so each input is loaded once per block.
+// register window w[k] = in[FP + t0 - jb - (JB-1) + k].  The next block's window is this one
+// moved down by JB entries, so it keeps the OPT-1 entries the two share and loads only JB new
+// ones.  Blocks go in pairs, unrolled so that the window slides by register renaming (no moves):
+// OPT+7 + 8 input loads per 16 taps instead of 2*(OPT+7).  Unrolling every block of the 64-tap
+// variant made its code three times larger and the pass slower.
 template<int OPT, int FP>
 __device__ __forceinline__ void fir_pass(float2 (&acc)[OPT], const float2 *__restrict__ in,
     const float2 *__restrict__ coef, int irpad, int t0)
 {
     constexpr int JB = 8;                       // taps per register-window block
-    for(int jb = 0;jb < irpad;jb += JB)
+    constexpr int W = OPT + JB - 1;
+    for(int jb = 0;jb < irpad;jb += 2*JB)
     {
-        float2 w[OPT+JB-1];
         const float2 *p = in + FP + t0 - jb - (JB-1);
+        float2 w[W];
         #pragma unroll
-        for(int k = 0;k < OPT+JB-1;++k) w[k] = p[k];
+        for(int k = 0;k < W;++k) w[k] = p[k];
         #pragma unroll
         for(int jj = 0;jj < JB;++jj)
         {
             const float2 c = coef[jb+jj];
+            #pragma unroll
+            for(int r = 0;r < OPT;++r)
+                acc[r] = fma2_rn(c, w[r - jj + (JB-1)], acc[r]);
+        }
+        if(jb + JB >= irpad) break;
+        #pragma unroll
+        for(int k = W-1;k >= JB;--k) w[k] = w[k-JB];
+        #pragma unroll
+        for(int k = 0;k < JB;++k) w[k] = p[k - JB];
+        #pragma unroll
+        for(int jj = 0;jj < JB;++jj)
+        {
+            const float2 c = coef[jb+JB+jj];
             #pragma unroll
             for(int r = 0;r < OPT;++r)
                 acc[r] = fma2_rn(c, w[r - jj + (JB-1)], acc[r]);
@@ -463,17 +481,92 @@ __device__ __forceinline__ void hold_end_sample(float *srcBuffer, uint32_t srcn,
     for(uint32_t k = best+1+t;k < tofill;k += GS) srcBuffer[k] = held;
 }
 
+// The 16-bit window copies of pack_window16, built straight from a one-run int16 span that the
+// bulk copy left at raw (sample 0 at halfword lead).  Span sample s becomes y = s + 32768, which
+// is the raw halfword XOR 0x8000, so an A word is the funnel of two neighbouring raw words,
+// XOR 0x80008000 (window position k sits at raw halfword k - kEdge - srcDelay + lead; the funnel
+// covers its parity).  Positions before the span, the history from prev (floats) and the
+// srcDelay zeros, are converted as pack_window16 converts them.  Only the A words are held
+// across the one barrier (the B copy overlaps the raw span): B word w = y(2w+1) | y(2w+2) << 16
+// is the funnel of A words w and w+1.  Each warp takes a run of 32*PER consecutive words, so a
+// lane gets word w+1 (and raw word w+1) from the next lane, lane 31 from lane 0 one step later.
+// Consecutive runs share one word: the earlier warp writes its A, the later one its B.  The
+// result equals what pack_window16 writes for the same window; positions past the span are
+// never read.
+template<int GS>
+__device__ __forceinline__ void pack_span16(float *win, const unsigned char *raw, uint32_t lead,
+    uint32_t srcDelay, uint32_t count, int t, int bar)
+{
+    constexpr int NW = (kResBuf + 8 + 1)/2;                    // words of one copy
+    constexpr int PER = (NW + GS - 1)/GS;                      // words per lane
+    static_assert((GS/32)*(32*PER - 1) >= NW + 1, "the warps' runs must cover every word");
+    const uint32_t lane = uint32_t(t) & 31u;
+    const uint32_t w0 = uint32_t(t >> 5)*(32u*PER - 1u) + lane;  // the lane's word at u = 0
+    const uint32_t lo = uint32_t(kEdge) + srcDelay;            // first position from the span
+    const uint32_t nw = (min(lo + count + 8u, uint32_t(kResBuf + 8)) + 1u)/2u;
+    // position 2w is raw halfword 2w - off: word w funnels raw words w - ceil(off/2) and the
+    // next by off's parity.  Raw word w holds positions 2w-1..2w+1, so it is loaded only when
+    // 2w+1 >= lo: words wholly before the span take their values from the masks below and read
+    // nothing (the srcDelay zeros may be being stored there).  Words past the span read other
+    // bytes of the group's storage (the phase table after the window), which the resampler's
+    // reach makes irrelevant.
+    const uint32_t off = lo - lead;
+    const uint32_t *rw = reinterpret_cast<const uint32_t*>(raw) - int((off + 1u) >> 1);
+    const uint32_t sh = (off & 1u)*16u;
+    uint32_t wa[PER];
+    #pragma unroll
+    for(int u = 0;u < PER;++u)
+    {
+        const uint32_t w = w0 + uint32_t(u)*32u;
+        wa[u] = (w <= nw && 2u*w + 1u >= lo) ? rw[w] : 0u;
+    }
+    #pragma unroll
+    for(int u = 0;u < PER;++u)
+    {
+        const uint32_t w = w0 + uint32_t(u)*32u;
+        uint32_t r1 = __shfl_sync(0xffffffffu, (u + 1 < PER && lane == 0u) ? wa[u + 1 < PER ? u + 1 : u] : wa[u],
+            (lane + 1u) & 31u);
+        if(u + 1 == PER && lane == 31u && w <= nw && 2u*w + 3u >= lo) r1 = rw[w + 1u];
+        uint32_t a = __funnelshift_r(wa[u], r1, sh) ^ 0x80008000u;
+        const int d = int(lo) - int(2u*w);                      // positions 2w, 2w+1 before lo: zeros
+        const uint32_t m = (d >= 1 ? 0x0000ffffu : 0u) | (d >= 2 ? 0xffff0000u : 0u);
+        a = (a & ~m) | (0x80008000u & m);
+        if(u == 0 && w < uint32_t(kEdge/2))                     // history
+            a = uint32_t(uint16_t(__float2int_rn(win[2u*w]*32768.0f) + 32768))
+                | (uint32_t(uint16_t(__float2int_rn(win[2u*w + 1u]*32768.0f) + 32768)) << 16);
+        wa[u] = a;
+    }
+    group_sync(bar, GS);                 // raw span and history read: the copies may overwrite them
+    uint32_t *pa = reinterpret_cast<uint32_t*>(win);
+    uint32_t *pb = pa + kPackB;
+    #pragma unroll
+    for(int u = 0;u < PER;++u)
+    {
+        const uint32_t w = w0 + uint32_t(u)*32u;
+        const uint32_t next = __shfl_sync(0xffffffffu, (u + 1 < PER && lane == 0u) ? wa[u + 1 < PER ? u + 1 : u] : wa[u],
+            (lane + 1u) & 31u);
+        if(w < nw)
+        {
+            if(u > 0 || lane > 0u || t < 32) pa[w] = wa[u];
+            if(u + 1 < PER || lane < 31u) pb[w] = __funnelshift_r(wa[u], next, 16u);
+        }
+    }
+}
+
 // TMA staging of the source span (the common case: a static mono int16 buffer, the span inside
 // the buffer, at most one loop wrap).  The span is one or two CONTIGUOUS runs of the buffer: one
 // thread issues a bulk copy (cp.async.bulk: global -> shared, completion on the group's
 // mbarrier) per run into the unused tail of the window storage; the group then converts from
 // shared memory.  Replaces ~1300 two-byte gathers per voice-chunk by one or two asynchronous
-// copies; the lines were pulled into L2 a round earlier.  Writes count samples to dst and
-// returns true, or returns false (nothing written) when the span does not qualify.
+// copies; the lines were pulled into L2 a round earlier.  Writes count samples to
+// win[kEdge+srcDelay..] and returns true, or returns false (nothing written) when the span does
+// not qualify.  With pack set, a one-run span goes straight into the 16-bit window copies
+// (pack_span16) and packed is set; otherwise the window is left as floats.
 template<int GS>
 __device__ __forceinline__ bool stage_span_tma(float *win, uint64_t *tmaBar, uint32_t &tmaPhase,
     const BufferRec &buf, uint32_t flags, bool isQueue, bool looping, uint32_t loopStart,
-    uint32_t loopEnd, uint32_t uintPos, uint32_t count, float *dst, int t, int bar)
+    uint32_t loopEnd, uint32_t uintPos, uint32_t srcDelay, uint32_t count, bool pack, bool &packed,
+    int t, int bar)
 {
     if(isQueue || buf.type != 1u || buf.channels != 1u || ((flags >> 16) & 0xffu) != 0u || count == 0u)
         return false;
@@ -505,6 +598,13 @@ __device__ __forceinline__ bool stage_span_tma(float *win, uint64_t *tmaBar, uin
     }
     mbar_wait(tmaBar, tmaPhase);
     tmaPhase ^= 1u;
+    if(pack && !run2)
+    {
+        pack_span16<GS>(win, raw1, lead1, srcDelay, count, t, bar);
+        packed = true;
+        return true;
+    }
+    float *dst = win + kEdge + srcDelay;
     const int16_t *r1 = reinterpret_cast<const int16_t*>(raw1) + lead1;
     const int16_t *r2 = reinterpret_cast<const int16_t*>(raw2) + lead2;
     constexpr int PERW = (kSrcSizeMax + GS - 1)/GS;
@@ -1005,7 +1105,7 @@ k_mix_voices(const MixParams P)
         VoiceRec &rec = P.voices[v];
         // one batch of vector loads for the scalar part of the record
         const uint4 *hp = reinterpret_cast<const uint4*>(&rec);
-        const uint4 h0 = hp[0], h1 = hp[1], h2 = hp[2], h3 = hp[3], h4 = hp[4];
+        const uint4 h0 = hp[0], h1 = hp[1], h2 = hp[2], h3 = hp[3];
         const uint32_t vstate = h0.x;
         if(voice_early_out(P, rec, v, vstate, h1, t)) continue;
         const uint32_t increment = h1.z;
@@ -1065,22 +1165,26 @@ k_mix_voices(const MixParams P)
             {
                 float *srcBuffer = S.win + kEdge;
                 bool winInt = false;       // every sample of this window came from a <=16-bit format
+                // the bsinc resamplers read the 16-bit copies when every sample is exact in them
+                const bool pack = resampler >= 4u && !(increment == 65536u && fracPos == 0u);
                 if(!haveBuffer) hold_end_sample<GS>(srcBuffer, srcn, t, bar);
                 else
                 {
                     const uint32_t uintPos = intPos < 0 ? 0u : uint32_t(intPos);
                     const uint32_t count = srcn - srcDelay;
-                    float *dst = srcBuffer + srcDelay;
                     for(uint32_t k = t;k < srcDelay;k += GS) srcBuffer[k] = 0.0f;
                     winInt = stage_span_tma<GS>(S.win, &S.tmaBar, tmaPhase, buf, flags, isQueue, looping,
-                            loopStart, loopEnd, uintPos, count, dst, t, bar)
+                            loopStart, loopEnd, uintPos, srcDelay, count, pack, packedWin, t, bar)
                         || gather_span<GS>(P, buf, flags, isQueue, qh, qitems, looping, loopStart, loopEnd,
-                            uintPos, count, dst, t, bar);
+                            uintPos, count, srcBuffer + srcDelay, t, bar);
                 }
                 group_sync(bar, GS);       // window complete
 
-                packedWin = resampler >= 4u && winInt && !(increment == 65536u && fracPos == 0u);
-                if(packedWin) pack_window16<GS>(S.win, srcn, t, bar);
+                if(pack && winInt && !packedWin)
+                {
+                    pack_window16<GS>(S.win, srcn, t, bar);
+                    packedWin = true;
+                }
                 resample_chunk<GS>(S.win, S.tabF, S.tabD, xs, loaded, dstn, increment, fracPos,
                     resampler, m, tapOff, ms, packedWin, t);
             }
@@ -1092,8 +1196,10 @@ k_mix_voices(const MixParams P)
         // ---- park, register dry mix, position / state write-back ----
         // fade bookkeeping (core/voice.cpp:1093-1112)
         const uint32_t counter = (flags & kVfFading) ? (n < 64u ? n : 64u) : 0u;
+        // the send mask is read here rather than held through the chunks: the parking
+        // variant has no register to spare there
         if(P.sendinfo)
-            park_voice<GS, CDR>(P, xs, v, h4.w, defer, isHrtf, playing, dirty, counter, t);
+            park_voice<GS, CDR>(P, xs, v, rec.send_mask, defer, isHrtf, playing, dirty, counter, t);
         // direct-path DoFilters (core/voice.cpp:943-946) with an inactive pair: clear()
         if(dfilt && !defer) filter_clear(*dfilt, t);
         if constexpr(CDR > 0)

@@ -247,7 +247,7 @@ def main():
             "transport": args.transport if world > 1 else None,
             "buffers": f"{nv} private device buffers per rank, {pool} distinct host waveforms", "direct_filters": bool(args.filters),
             "ms_per_update": ms_update, "mix_kernel_ms_rank0": float(np.mean(mix)),
-            "stage_us_rank0": dict(zip(["clear", "voices", "filters+deferred", "reduce", "dry_bus", "sends",
+            "stage_us_rank0": dict(zip(["clear", "voices", "filters+fir/deferred", "reduce", "dry_bus", "sends",
                                         "effects", "post"],
                                        [round(float(x) * 1e3, 1) for x in np.mean(stages, axis=0)]))
             if stages else None,
