@@ -9,13 +9,15 @@
 //      resampled line is parked in HBM (xscratch) or, on devices with at most 4 dry
 //      channels, mixed into register accumulators of the dry bus; on those devices
 //      k_mix_deferred mixes the lines of voices with an active direct filter once filtered,
-//   2. k_hrtf_fir (HRTF devices): per parked HRTF voice, builds the per-ear, gain-ramped FIR
+//   2. k_hrtf_fir (HRTF devices): per parked HRTF voice, bulk-copied into shared memory one
+//      voice ahead, builds the per-ear, gain-ramped FIR
 //      inputs (DoHrtfMix, core/voice.cpp:827-902; MixHrtfBlend/MixHrtf, hrtfbase.h:17-89)
 //      and runs the HRIR FIR with the outputs held in registers ACROSS all voices of the
 //      group (the cross-voice reduction of `Accum[i+j] += ...` happens in registers),
 // and the accumulating kernels store one partial row per CTA; k_reduce_* sums the rows in a
 // fixed order (deterministic output).
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -269,15 +271,25 @@ struct alignas(16) GroupSmem {
     uint32_t claimed;                   // order index the group claimed last (parking variant)
 };
 
-// Shared-memory carve-up of one voice group of k_hrtf_fir.
+// What k_hrtf_fir bulk-copies for one voice: [History | resampled line] and the target HRIR,
+// plus the old HRIR when the voice is dirty.
+struct alignas(16) FirStage {
+    float x[kHist + kLine];
+    float2 coefT[kHrirLen], coefO[kHrirLen];
+};
+static_assert(offsetof(VoiceRec, hist) % 16 == 0 && sizeof(VoiceRec) % 16 == 0,
+    "VoiceRec::hist is a bulk-copy source: 16-byte aligned");
+
+// Shared-memory carve-up of one voice group of k_hrtf_fir.  The stage buffers alternate
+// between voices: one is filled for the group's next voice while the other is read.
 template<int GS, int OPT, int FP>
 struct alignas(16) FirSmem {
     static constexpr int kLLen = FP + OPT*GS;           // FIR input incl. front zero pad
     static constexpr int kOLen = FP + kHist + FP + 32;  // old-coefficient pass input
     float2 lLR[kLLen];                  // {left, right} per input sample
     float2 oLR[kOLen];
-    float x[kHist + kLine];             // [History | resampled line]
-    float2 coefT[kHrirLen], coefO[kHrirLen];
+    FirStage st[2];
+    uint64_t bar[2];                    // mbarrier of each stage buffer's bulk copies
 };
 
 // Both ears' MACs: {a.x*b.x + c.x, a.y*b.y + c.y}, each one fused multiply-add (round to
@@ -1273,10 +1285,42 @@ k_mix_deferred(const MixParams P)
 // registers ACROSS all voices of the group (the cross-voice reduction of `Accum[i+j] += ...`
 // happens in registers, not memory).  Voices are assigned statically in the mixing order and
 // each CTA stores one partial row; k_reduce_rows sums the rows in a fixed order
-// (deterministic output).
+// (deterministic output).  A group's inputs for its next voice are bulk-copied into its second
+// stage buffer while the current voice is built and filtered.
 //   OPT/FP : FIR outputs per thread / front pad (17/64 for ir<=64, 19/128 for ir<=128)
 // ---------------------------------------------------------------------------
 constexpr int kFirGS = 64, kFirGroups = 2, kFirCtasPerSm = 4;
+
+// First order slot from oi on, in steps of stride, whose voice was parked for the HRIR FIR
+// (kSiHrtf), with that voice and its sendinfo; P.num_order or more when there is none.
+__device__ __forceinline__ uint32_t next_hrtf_voice(const MixParams &P, uint32_t oi, uint32_t stride,
+    uint32_t &v, uint32_t &info)
+{
+    for(;oi < P.num_order;oi += stride)
+    {
+        v = P.order[oi];
+        info = P.sendinfo[v];
+        if(info & kSiHrtf) break;
+    }
+    return oi;
+}
+
+// One thread fills stage buffer B with voice v's History, line and HRIR(s) by bulk copies that
+// complete on bar.  A bulk copy moves a multiple of 16 bytes, so the line's last n%4 samples are
+// left to plain loads.
+__device__ __forceinline__ void fir_stage_issue(const MixParams &P, FirStage &B, uint64_t *bar,
+    uint32_t v, uint32_t info, uint32_t n)
+{
+    const uint32_t lineBytes = (n & ~3u)*4u, irBytes = P.ir_pad*8u;
+    const bool dirty = (info & kSiDirty) != 0;
+    const float *line = ((info & kSiDeferred) ? P.dline : P.xscratch) + size_t(v)*kLine;
+    fence_proxy_async_smem();            // the group's generic accesses to B come first
+    mbar_expect_tx(bar, kHist*4u + lineBytes + (dirty ? 2u : 1u)*irBytes);
+    bulk_g2s(B.x, P.voices[v].hist, kHist*4u, bar);
+    if(lineBytes) bulk_g2s(B.x + kHist, line, lineBytes, bar);
+    bulk_g2s(B.coefT, P.hrtf_tgt + size_t(v)*P.ir_pad, irBytes, bar);
+    if(dirty) bulk_g2s(B.coefO, P.hrtf_old + size_t(v)*P.ir_pad, irBytes, bar);
+}
 
 template<int OPT, int FP>
 __global__ void __launch_bounds__(kFirGS*kFirGroups, kFirCtasPerSm)
@@ -1296,37 +1340,44 @@ k_hrtf_fir(const MixParams P)
     #pragma unroll
     for(int r = 0;r < OPT;++r) acc[r] = make_float2(0.0f, 0.0f);
 
+    // the FIR input's front pad and the samples past the update's end are zero for every voice
+    for(int i = t;i < FP;i += GS) S.lLR[i] = make_float2(0.0f, 0.0f);
+    for(int i = FP + int(n) + t;i < Smem::kLLen;i += GS) S.lLR[i] = make_float2(0.0f, 0.0f);
+    if(t == 0) { mbar_init(&S.bar[0], 1u); mbar_init(&S.bar[1], 1u); mbar_fence_init(); }
+    group_sync(bar, GS);
+
     const uint32_t stride = gridDim.x*GROUPS;
-    for(uint32_t oi = blockIdx.x*GROUPS + g;oi < P.num_order;oi += stride)
+    uint32_t v = 0u, info = 0u;
+    uint32_t oi = next_hrtf_voice(P, blockIdx.x*GROUPS + g, stride, v, info);
+    if(t == 0 && oi < P.num_order) fir_stage_issue(P, S.st[0], &S.bar[0], v, info, n);
+    uint32_t parity = 0u;                    // bit b: parity of stage buffer b's next completion
+    for(int b = 0;oi < P.num_order;b ^= 1)
     {
-        const uint32_t v = P.order[oi];
-        const uint32_t info = P.sendinfo[v];
-        if(!(info & kSiHrtf)) continue;
         VoiceRec &rec = P.voices[v];
         const uint4 *hp = reinterpret_cast<const uint4*>(&rec);
-        const uint4 h3 = hp[3], h4 = hp[4];
+        const uint4 h3 = hp[3], h4 = hp[4];     // in flight during the look-ahead's loads
+
+        // the group's next voice is copied into the other stage buffer while this one mixes
+        // (the previous voice's reads of it ended at the last barrier)
+        uint32_t vN = 0u, infoN = 0u;
+        const uint32_t oiN = next_hrtf_voice(P, oi + stride, stride, vN, infoN);
+        if(t == 0 && oiN < P.num_order) fir_stage_issue(P, S.st[b^1], &S.bar[b^1], vN, infoN, n);
+
+        FirStage &B = S.st[b];
         const bool playing = (info & kSiPlaying) != 0;
         const bool dirty = (info & kSiDirty) != 0;
         const uint32_t counter = (info >> 8) & 0xffu;
 
-        // ---- stage [History | line] and both coefficient sets ----
+        // ---- the line's last n%4 samples, which the bulk copy leaves out ----
         const float *line = ((info & kSiDeferred) ? P.dline : P.xscratch) + size_t(v)*kLine;
-        for(int k = t;k < kHist;k += GS) S.x[k] = rec.hist[k];
-        for(uint32_t k = t;k < n;k += GS) S.x[kHist + k] = line[k];
-        const float2 *ct = P.hrtf_tgt + size_t(v)*P.ir_pad;
-        const float2 *co = P.hrtf_old + size_t(v)*P.ir_pad;
-        for(int k = t;k < int(P.ir_pad);k += GS)
-        {
-            const float2 c = ct[k];
-            S.coefT[k] = c;
-            S.coefO[k] = dirty ? co[k] : c;
-        }
-        group_sync(bar, GS);
-
+        for(uint32_t k = (n & ~3u) + t;k < n;k += GS) B.x[kHist + k] = line[k];
+        mbar_wait(&S.bar[b], (parity >> b) & 1u);
+        parity ^= 1u << b;
+        if(n & 3u) group_sync(bar, GS);
 
         // DoHrtfMix (core/voice.cpp:827-902), outPos == 0
         if(playing)
-            for(int k = t;k < kHist;k += GS) rec.hist[k] = S.x[n + k];
+            for(int k = t;k < kHist;k += GS) rec.hist[k] = B.x[n + k];
         uint32_t oD0 = h4.x, oD1 = h4.y;
         float oGain = __uint_as_float(h4.z);
         const uint32_t tD0 = h3.y, tD1 = h3.z;
@@ -1350,28 +1401,27 @@ k_hrtf_fir(const MixParams P)
         const uint32_t todo = n - fademix;
         const float step2 = todo ? (targetGain - gainA) / float(todo) : 0.0f;
 
-        const float *hs = S.x;                                // [History | samples]
-        for(int i = t;i < Smem::kLLen;i += GS)
+        // FIR input sample s at lLR[FP + s]; the pad and the tail stay zero from the start
+        const float *hs = B.x;                                // [History | samples]
+        float2 *in = S.lLR + FP;
+        for(uint32_t s = t;s < fademix;s += GS)               // the fade (at most 64 samples)
         {
-            const int s = i - FP;                             // input sample index
-            float l = 0.0f, r = 0.0f;
-            if(s >= 0 && s < int(n))
+            const float gnew = (newOn && s >= 1u) ? blendNewStep*float(s) : 0.0f;
+            float l = hs[kHist - tD0 + s] * gnew;
+            float r = hs[kHist - tD1 + s] * gnew;
+            if(sameFilter && oldOn)
             {
-                float gnew;
-                if(uint32_t(s) < fademix)
-                    gnew = (newOn && s >= 1) ? blendNewStep*float(s) : 0.0f;
-                else
-                    gnew = gainA + step2*float(uint32_t(s) - fademix);
-                l = hs[kHist - tD0 + s] * gnew;
-                r = hs[kHist - tD1 + s] * gnew;
-                if(sameFilter && oldOn && uint32_t(s) < fademix)
-                {
-                    const float gold = oldStep*float(fademix - uint32_t(s));
-                    l += hs[kHist - oD0 + s] * gold;
-                    r += hs[kHist - oD1 + s] * gold;
-                }
+                const float gold = oldStep*float(fademix - s);
+                l += hs[kHist - oD0 + s] * gold;
+                r += hs[kHist - oD1 + s] * gold;
             }
-            S.lLR[i] = make_float2(l, r);
+            in[s] = make_float2(l, r);
+        }
+        const float *xl = hs + kHist - tD0, *xr = hs + kHist - tD1;
+        for(uint32_t s = fademix + t;s < n;s += GS)           // the steady ramp
+        {
+            const float gnew = gainA + step2*float(s - fademix);
+            in[s] = make_float2(xl[s] * gnew, xr[s] * gnew);
         }
         const bool oldPass = !sameFilter && oldOn;
         if(oldPass)
@@ -1389,35 +1439,17 @@ k_hrtf_fir(const MixParams P)
             }
         group_sync(bar, GS);
 
-        // software prefetch for the voices this group mixes next (overlaps the FIR): the
-        // record and HRIR two voices ahead, the parked line one voice ahead
-        {
-            const uint32_t o2 = oi + 2u*stride, o1 = oi + stride;
-            const uint32_t v2 = o2 < P.num_order ? P.order[o2] : 0xffffffffu;
-            const uint32_t v1 = o1 < P.num_order ? P.order[o1] : 0xffffffffu;
-            if(v2 < P.max_voices)
-            {
-                if(t < 5) prefetch_l2(reinterpret_cast<const char*>(&P.voices[v2]) + t*128);
-                else if(t < 5 + int((P.ir_pad*8u + 127u)/128u))
-                    prefetch_l2(reinterpret_cast<const char*>(P.hrtf_tgt + size_t(v2)*P.ir_pad) + (t-5)*128);
-            }
-            if(v1 < P.max_voices && t < int(kLine*sizeof(float)/128u))
-            {
-                const float *nl = ((P.sendinfo[v1] & kSiDeferred) ? P.dline : P.xscratch) + size_t(v1)*kLine;
-                prefetch_l2(reinterpret_cast<const char*>(nl) + t*128);
-            }
-        }
-
         const int irpad = int(P.ir_pad);
-        fir_pass<OPT, FP>(acc, S.lLR, S.coefT, irpad, t0);
-        if(oldPass && t0 < int(kHist) + irpad)
-            fir_pass<OPT, FP>(acc, S.oLR, S.coefO, irpad, t0);
+        fir_pass<OPT, FP>(acc, S.lLR, B.coefT, irpad, t0);
+        if(oldPass && t0 < int(kHist) + irpad)      // the old HRIR is the target one unless dirty
+            fir_pass<OPT, FP>(acc, S.oLR, dirty ? B.coefO : B.coefT, irpad, t0);
         if(t == 0)
         {
             rec.old_delay0 = tD0; rec.old_delay1 = tD1;
             rec.old_gain = targetGain;
         }
-        group_sync(bar, GS);               // smem free for the next voice
+        group_sync(bar, GS);               // lLR, oLR and stage buffer b free for the next voices
+        oi = oiN; v = vN; info = infoN;
     }
 
     // ---- one partial row per CTA: the groups' register accumulators are summed through
