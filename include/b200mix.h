@@ -542,6 +542,48 @@ B200MIX_API int b200mix_calc_voice_bformat(const b200mix_source_props *props,
 B200MIX_API int b200mix_voice_queue(b200mix_device *dev, uint32_t voice, uint32_t count,
     const uint32_t *buffers, uint32_t loop_index);
 
+/* Callback buffers (AL_SOFT_callback_buffer, alBufferCallbackSOFT): the application supplies
+ * the samples while the source plays.  b200mix_buffer_callback makes `buffer` such a buffer
+ * (BufferStorage::mCallback / mUserData, al/buffer.cpp:447-511).  A voice whose `buffer` names
+ * it is a callback voice: STATIC must be clear, its queue is ignored, looping too, and it joins
+ * with B200MIX_VF_RESET (InitVoice, al/source.cpp:659-662).  All channel voices of one source
+ * share the buffer and must agree on step, position and state (else voices_update fails with
+ * B200MIX_ERR_INVALID).  B200MIX_VF_RESET on any of them returns the state to 0,0,0.
+ *
+ * The library calls `callback` on the calling thread inside b200mix_render, _render_device,
+ * _render_interleaved and _render_begin, before the update is launched, and nowhere else.  It
+ * makes the reference's calls (core/voice.cpp:726-753): per chunk of the update, the missing
+ * whole blocks, written at storage + num_blocks*bytes_per_block; a short return ends the
+ * stream.  After the update it drops the blocks the voice has passed by moving the rest to
+ * the front of `storage` (core/voice.cpp:1155-1180), so `storage` always holds the bytes the
+ * reference's buffer holds.  When the stream runs out the voice ends like a static voice at
+ * the end of its buffer (Stopping, no buffer).  IMA4 / MSADPCM blocks are decoded on the host
+ * as b200mix_buffer_data_adpcm does.  num_blocks / block_offset / stopped give the state to
+ * continue from (Voice::mNumCallbackBlocks, mCallbackBlockOffset, CallbackStopped; 0,0,0 for a
+ * new stream): to carry a stream over to a new device, register the buffer there after the
+ * voices' RESET update.  storage_bytes must be at least the reference's callback storage
+ * (al/buffer.cpp:468-473: ceil(((1024 + 256)*10 + 24) / samples_per_block) blocks), which no
+ * request passes.  At most 16 channels.  Callback voices are updated with b200mix_voices_update
+ * only: b200mix_sources_update refuses them (B200MIX_ERR_UNSUPPORTED), since it computes the
+ * step on the GPU, out of the planner's sight.  A callback buffer's voices must live on the
+ * device that registered it (sharded sets add no special handling).
+ * buffer_data / buffer_free on the id end its callback registration (refused while a voice
+ * plays it). */
+typedef int (*b200mix_callback_fn)(void *userptr, void *sampledata, int numbytes); /* ALBUFFERCALLBACKTYPESOFT */
+typedef struct b200mix_callback_buffer {
+    uint32_t struct_size;
+    uint32_t sample_type, channels;                 /* enum b200mix_sample_type, incl. IMA4 / MSADPCM */
+    uint32_t samples_per_block, bytes_per_block;    /* Voice::mSamplesPerBlock / mBytesPerBlock (1 and the
+                                                       frame size for PCM) */
+    b200mix_callback_fn callback; void *userptr;    /* VoiceBufferItem::mCallback / mUserData */
+    void *storage; size_t storage_bytes;            /* the bytes the callback writes into (BufferStorage) */
+    uint32_t num_blocks, block_offset, stopped;     /* state to resume from; 0,0,0 for a new stream */
+} b200mix_callback_buffer;
+B200MIX_API int b200mix_buffer_callback(b200mix_device *dev, uint32_t buffer, const b200mix_callback_buffer *cb);
+/* The buffer's state after the last update (and its callbacks). */
+B200MIX_API int b200mix_buffer_callback_state(b200mix_device *dev, uint32_t buffer,
+    uint32_t *num_blocks, uint32_t *block_offset, uint32_t *stopped);
+
 /* Direct and send filters: DoFilters -> BiquadInterpFilter::dualProcess
  * (core/voice.cpp:255-268, core/filters/biquad.cpp:254-343).  One entry is the RESULT of
  * the parameter stage's filter block for one path of one voice (alc/alu.cpp:1619-1656):

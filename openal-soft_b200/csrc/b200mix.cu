@@ -29,6 +29,7 @@
 #include "resampler_tables.hpp"
 #include "hrtf_store.hpp"
 #include "adpcm.hpp"
+#include "callback_plan.hpp"
 
 using namespace b200mix;
 
@@ -224,7 +225,36 @@ struct b200mix_device {
     uint32_t reverb_seq{0};          // update counter of k_reverb_process' early/late hand-off (24 bits used)
     uint32_t *d_claim{nullptr};      // voice claim counters of the parking k_mix_voices
     int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
+
+    // callback buffers (b200mix_buffer_callback): the registrations (plan slots), the host's
+    // mirror of the voices that play them (positions advance by the same arithmetic as on the
+    // device, so planning needs no read-back), and the pinned arenas their samples travel in,
+    // alternating so that one can be filled while the other's copy is in flight
+    struct CbBuf {
+        bool used{false};
+        uint32_t buffer{0};
+        b200mix_callback_buffer cb{};
+        cbplan::State st{};
+        uint32_t frame_bytes{0};             // bytes per sample frame in the arena (int16 for ADPCM)
+    };
+    std::vector<CbBuf> cbs;
+    std::vector<int32_t> cb_of_buffer;       // buffer id -> plan slot or -1
+    struct CbVoice { int32_t slot{-1}; cbplan::Voice v{}; };
+    std::vector<CbVoice> cbv;                // per voice
+    uint32_t cb_bound{0};                    // voices bound to a callback buffer
+    char *h_cb[2]{}; size_t h_cb_cap[2]{}; cudaEvent_t cb_done[2]{}; bool cb_busy[2]{}; int cb_idx{0};
+    char *d_cb{nullptr}; size_t d_cb_cap{0};
+    void *d_cb_zero{nullptr};                // zeros behind every callback buffer's own record
+    std::vector<int32_t> cb_reps;            // per slot: the voice the update is planned from (-1: none)
+    std::vector<std::vector<uint32_t>> cb_members;   // per slot: its other mixing voices
+    struct CbWork { cbplan::State start; cbplan::Loads loads; size_t region{0}, bytes{0}; };
+    std::vector<CbWork> cb_work;             // per slot, for the update being planned
 };
+
+namespace {
+constexpr uint32_t kCbMaxChannels = 16;      // a callback buffer's frame is at most 16*8 bytes
+constexpr size_t kCbPad = 256;               // zero bytes that cover one such frame
+}
 
 namespace {
 
@@ -321,7 +351,7 @@ extern "C" {
 static void shard_release(b200mix_device *d);
 static int ensure_filters(b200mix_device *d);
 
-uint32_t b200mix_version(void) { return (1u<<16) | 1u; }
+uint32_t b200mix_version(void) { return (1u<<16) | 2u; }
 
 const char *b200mix_last_error(const b200mix_device *dev)
 { return dev ? dev->error.c_str() : g_create_error.c_str(); }
@@ -529,7 +559,8 @@ void b200mix_destroy(b200mix_device *d)
     if(!d) return;
     if(d->stream) cudaStreamSynchronize(d->stream);
     shard_release(d);
-    for(auto &b : d->h_buffers) if(b.data) cudaFree(const_cast<void*>(b.data));
+    for(auto &b : d->h_buffers) if(b.data && !b.pad) cudaFree(const_cast<void*>(b.data));
+    cudaFree(d->d_cb_zero);
     for(int i = 0;i < 3;++i) cudaFree(d->d_bsinc[i]);
     for(int i = 0;i < 2;++i) cudaFree(d->d_cubic[i]);
     cudaFree(d->d_voices); cudaFree(d->d_buffers); cudaFree(d->d_hrtf_tgt); cudaFree(d->d_hrtf_old);
@@ -562,6 +593,12 @@ void b200mix_destroy(b200mix_device *d)
     cudaFree(d->d_src);
     if(d->src_done) cudaEventDestroy(d->src_done);
     if(d->stage_done) cudaEventDestroy(d->stage_done);
+    for(int i = 0;i < 2;++i)
+    {
+        if(d->h_cb[i]) cudaFreeHost(d->h_cb[i]);
+        if(d->cb_done[i]) cudaEventDestroy(d->cb_done[i]);
+    }
+    cudaFree(d->d_cb);
     if(d->ev_mix0) cudaEventDestroy(d->ev_mix0);
     if(d->ev_mix1) cudaEventDestroy(d->ev_mix1);
     for(cudaEvent_t e : d->ev_stage) if(e) cudaEventDestroy(e);
@@ -620,6 +657,108 @@ int b200mix_set_ambi_decoder(b200mix_device *d, uint32_t in_channels, const floa
     return B200MIX_OK;
 }
 
+// Voices that play callback plan slot s (playing or stopping).
+static uint32_t cb_slot_voices(const b200mix_device *d, int32_t s)
+{
+    uint32_t n = 0;
+    for(uint32_t v = 0;v < d->cbv.size() && v < d->voice_hi;++v)
+        n += d->cbv[v].slot == s && (d->cbv[v].v.state == 1u || d->cbv[v].v.state == 2u);
+    return n;
+}
+
+// Ends the callback registration of `buffer` (if any); refused while a voice plays it.
+static int cb_unregister(b200mix_device *d, uint32_t buffer, const char *what)
+{
+    if(d->cb_of_buffer.empty() || d->cb_of_buffer[buffer] < 0) return B200MIX_OK;
+    const int32_t s = d->cb_of_buffer[buffer];
+    if(cb_slot_voices(d, s))
+    { d->error = std::string(what) + ": the callback buffer is played by a voice; stop it first"; return B200MIX_ERR_INVALID; }
+    for(auto &cv : d->cbv)
+        if(cv.slot == s) { cv.slot = -1; --d->cb_bound; }
+    d->cbs[size_t(s)] = b200mix_device::CbBuf{};
+    d->cb_of_buffer[buffer] = -1;
+    d->h_buffers[buffer] = BufferRec{};
+    CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &d->h_buffers[buffer], sizeof(BufferRec),
+        cudaMemcpyHostToDevice, d->stream));
+    return B200MIX_OK;
+}
+
+int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_callback_buffer *cb)
+{
+    if(!d) return B200MIX_ERR_INVALID;
+    const b200mix_device_desc &dd = d->desc;
+    if(buffer >= dd.max_buffers || !cb || cb->struct_size != sizeof(b200mix_callback_buffer) || !cb->callback
+        || cb->sample_type > B200MIX_FMT_MSADPCM || cb->channels < 1 || !cb->storage
+        || cb->samples_per_block < 1 || cb->bytes_per_block < 1)
+    { d->error = "buffer_callback: bad arguments"; return B200MIX_ERR_INVALID; }
+    static const uint32_t sz[] = {1, 2, 4, 4, 8, 1, 1};
+    const bool adpcm = cb->sample_type >= B200MIX_FMT_IMA4;
+    const bool ms = cb->sample_type == B200MIX_FMT_MSADPCM;
+    if(adpcm ? (cb->channels > 2 || !AdpcmBlockValid(ms, cb->samples_per_block)
+                || cb->bytes_per_block != AdpcmBlockBytes(ms, cb->channels, cb->samples_per_block))
+             : (cb->samples_per_block != 1u || cb->bytes_per_block != cb->channels*sz[cb->sample_type]))
+    { d->error = "buffer_callback: block size does not match the format"; return B200MIX_ERR_INVALID; }
+    if(cb->channels > kCbMaxChannels)
+    { d->error = "buffer_callback: more than 16 channels"; return B200MIX_ERR_UNSUPPORTED; }
+    // PrepareCallback's size (al/buffer.cpp:468-473): MixerLineSize*MaxPitch + MaxResamplerEdge
+    // samples in whole blocks.  No request of the reference's chunk loop passes it, so the
+    // callbacks of an update never stop half way.
+    const uint64_t lineBlocks = ((1024u + 256u)*10u + 24u + cb->samples_per_block - 1u) / cb->samples_per_block;
+    if(cb->storage_bytes < lineBlocks*cb->bytes_per_block)
+    { d->error = "buffer_callback: storage smaller than the reference's callback storage"; return B200MIX_ERR_INVALID; }
+    if(uint64_t(cb->num_blocks)*cb->bytes_per_block > cb->storage_bytes || cb->stopped > 1u)
+    { d->error = "buffer_callback: state outside the storage"; return B200MIX_ERR_INVALID; }
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
+    if(!d->d_cb_zero)
+        if(int rc = dev_alloc(d, d->d_cb_zero, kCbPad)) return rc;
+    if(d->cb_of_buffer.empty())
+    {
+        d->cb_of_buffer.assign(dd.max_buffers, -1);
+        d->cbv.assign(dd.max_voices, b200mix_device::CbVoice{});
+    }
+    BufferRec &h = d->h_buffers[buffer];
+    int32_t s = d->cb_of_buffer[buffer];
+    if(s < 0)
+    {
+        if(h.data && d->h_bufrefs[buffer])
+        { d->error = "buffer_callback: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
+        if(h.data)
+        {
+            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            cudaFree(const_cast<void*>(h.data));
+        }
+        for(s = 0;size_t(s) < d->cbs.size() && d->cbs[size_t(s)].used;++s) {}
+        if(size_t(s) == d->cbs.size()) d->cbs.emplace_back();
+        d->cb_of_buffer[buffer] = s;
+    }
+    b200mix_device::CbBuf &c = d->cbs[size_t(s)];
+    c.used = true; c.buffer = buffer; c.cb = *cb;
+    c.st = cbplan::State{cb->num_blocks, cb->block_offset, cb->stopped};
+    c.frame_bytes = cb->channels*(adpcm ? 2u : sz[cb->sample_type]);
+    // the kernel reads the samples from the update's arena: the record carries the format, and
+    // zeros to read should a voice ever meet it without a plan
+    h = BufferRec{};
+    h.data = d->d_cb_zero;
+    h.type = adpcm ? uint32_t(B200MIX_FMT_I16) : cb->sample_type;
+    h.channels = cb->channels;
+    h.pad = uint32_t(s) + 1u;
+    CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec), cudaMemcpyHostToDevice, d->stream));
+    return B200MIX_OK;
+}
+
+int b200mix_buffer_callback_state(b200mix_device *d, uint32_t buffer, uint32_t *num_blocks,
+    uint32_t *block_offset, uint32_t *stopped)
+{
+    if(!d) return B200MIX_ERR_INVALID;
+    if(buffer >= d->desc.max_buffers || d->cb_of_buffer.empty() || d->cb_of_buffer[buffer] < 0)
+    { d->error = "buffer_callback_state: not a callback buffer"; return B200MIX_ERR_INVALID; }
+    const cbplan::State &st = d->cbs[size_t(d->cb_of_buffer[buffer])].st;
+    if(num_blocks) *num_blocks = st.num_blocks;
+    if(block_offset) *block_offset = st.block_offset;
+    if(stopped) *stopped = st.stopped;
+    return B200MIX_OK;
+}
+
 int b200mix_buffer_data(b200mix_device *d, uint32_t buffer, uint32_t sample_type, uint32_t channels,
     uint32_t frames, const void *data, size_t bytes)
 {
@@ -627,6 +766,7 @@ int b200mix_buffer_data(b200mix_device *d, uint32_t buffer, uint32_t sample_type
     static const size_t sz[] = {1, 2, 4, 4, 8, 1, 1};
     if(buffer >= d->desc.max_buffers || sample_type > B200MIX_FMT_ALAW || channels < 1 || !data)
     { d->error = "buffer_data: bad arguments"; return B200MIX_ERR_INVALID; }
+    if(int rc = cb_unregister(d, buffer, "buffer_data")) return rc;
     const size_t need = size_t(frames)*channels*sz[sample_type];
     if(bytes < need) { d->error = "buffer_data: short data"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
@@ -674,6 +814,7 @@ int b200mix_buffer_free(b200mix_device *d, uint32_t buffer)
 {
     if(!d || buffer >= d->desc.max_buffers) return B200MIX_ERR_INVALID;
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
+    if(int rc = cb_unregister(d, buffer, "buffer_free")) return rc;
     BufferRec &h = d->h_buffers[buffer];
     if(h.data && d->h_bufrefs[buffer])
     { d->error = "buffer_free: the buffer is attached to an active voice; stop the voice first"; return B200MIX_ERR_INVALID; }
@@ -1185,6 +1326,33 @@ int b200mix_hrtf_attach(b200mix_device *d, const b200mix_hrtf *h)
 static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
     const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains);
 
+// The voices of each callback buffer are the channels of one source: cb_reps[slot] = the first one
+// that mixes this update (-1: none), cb_members[slot] the others, which must agree with it on what
+// the planner reads.  One pass over the voices.
+static int cb_group(b200mix_device *d)
+{
+    std::vector<int32_t> &reps = d->cb_reps;
+    reps.assign(d->cbs.size(), -1);
+    d->cb_members.resize(d->cbs.size());
+    for(auto &m : d->cb_members) m.clear();
+    for(uint32_t v = 0;v < d->voice_hi;++v)
+    {
+        const b200mix_device::CbVoice &cv = d->cbv[v];
+        if(cv.slot < 0 || (cv.v.state != 1u && cv.v.state != 2u)) continue;
+        int32_t &r = reps[size_t(cv.slot)];
+        if(r < 0) { r = int32_t(v); continue; }
+        const cbplan::Voice &a = d->cbv[size_t(r)].v, &b = cv.v;
+        if(a.pos != b.pos || a.frac != b.frac || a.step != b.step || a.state != b.state
+            || a.have_buffer != b.have_buffer)
+        {
+            d->error = "voices_update: voices sharing a callback buffer disagree on step, position or state";
+            return B200MIX_ERR_INVALID;
+        }
+        d->cb_members[size_t(cv.slot)].push_back(v);
+    }
+    return B200MIX_OK;
+}
+
 int b200mix_voices_update(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
     const float *hrtf_coeffs, const float *dry_gains, const float *send_gains)
 {
@@ -1228,9 +1396,16 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         // relies on it
         if(p.step > (10u << 16))
         { d->error = "voices_update: step above MaxPitch<<16"; return B200MIX_ERR_INVALID; }
+        // callback voice: plays a buffer made by b200mix_buffer_callback
+        const int32_t cbSlot = (!(p.flags & B200MIX_VF_STOPPED) && !nobuf && !d->cb_of_buffer.empty())
+            ? d->cb_of_buffer[p.buffer] : -1;
+        if(cbSlot >= 0 && (p.flags & B200MIX_VF_STATIC))
+        { d->error = "voices_update: a callback buffer is not static (IsCallback)"; return B200MIX_ERR_INVALID; }
+        if(cbSlot >= 0 && d->cbv[p.voice].slot != cbSlot && !(p.flags & B200MIX_VF_RESET))
+        { d->error = "voices_update: a voice starts a callback buffer with B200MIX_VF_RESET"; return B200MIX_ERR_INVALID; }
         if(!(p.flags & B200MIX_VF_STOPPED))
         {
-            if(nobuf) { /* nothing to read */ }
+            if(nobuf || cbSlot >= 0) { /* nothing to read / read from the update's arena */ }
             else if(p.flags & B200MIX_VF_STATIC)
             {
                 const BufferRec &hb = d->h_buffers[p.buffer];
@@ -1294,6 +1469,30 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
             d->h_active[p.voice] = act; d->h_cost[p.voice] = cost;
         }
         d->voice_hi = std::max(d->voice_hi, p.voice + 1u);
+        if(!d->cbv.empty())
+        {
+            // the planner's mirror of the voice: what k_apply_updates does to its record
+            b200mix_device::CbVoice &cv = d->cbv[p.voice];
+            const int32_t slot = nobuf && !(p.flags & B200MIX_VF_STOPPED) ? cv.slot : cbSlot;
+            if(slot != cv.slot)
+            {
+                d->cb_bound = d->cb_bound + (slot >= 0) - (cv.slot >= 0);
+                cv.slot = slot;
+            }
+            if(slot >= 0)
+            {
+                cbplan::Voice &m = cv.v;
+                if(p.flags & B200MIX_VF_RESET)
+                {
+                    m.pos = p.position; m.frac = p.position_frac; m.have_buffer = true;
+                    d->cbs[size_t(slot)].st = cbplan::State{};
+                }
+                if(p.flags & B200MIX_VF_STOPPING) m.state = 2u;
+                else if(p.flags & B200MIX_VF_PLAYING) m.state = 1u;
+                m.step = p.step;
+                if(nobuf) m.have_buffer = false;
+            }
+        }
         {
             const uint32_t nb = (!(p.flags & B200MIX_VF_STOPPED) && (p.flags & B200MIX_VF_STATIC) && !nobuf)
                 ? p.buffer : B200MIX_NO_SLOT;
@@ -1308,6 +1507,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         if((p.flags & B200MIX_VF_RESET) && !d->h_dfilt.empty() && d->h_dfilt[p.voice])
         { d->h_dfilt[p.voice] = 0; d->order2_dirty = true; }
     }
+    if(d->cb_bound)
+        if(int rc = cb_group(d)) return rc;
     ApplyParams A{};
     A.voices = d->d_voices; A.updates = reinterpret_cast<const VoiceUpdate*>(d->d_arena);
     size_t off = align16(size_t(n)*sizeof(VoiceUpdate));
@@ -1392,6 +1593,10 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
         { d->error = "sources_update: voice/buffer/resampler out of range"; return B200MIX_ERR_INVALID; }
         if((p.flags & B200MIX_VF_LOOPING) && p.loop_end <= p.loop_start)
         { d->error = "sources_update: empty loop"; return B200MIX_ERR_INVALID; }
+        // callback voices are planned from the steps b200mix_voices_update gives; this stage
+        // computes them on the device, where the planner cannot see them
+        if(!(p.flags & B200MIX_VF_STOPPED) && !d->cb_of_buffer.empty() && d->cb_of_buffer[p.buffer] >= 0)
+        { d->error = "sources_update: callback buffers play through b200mix_voices_update"; return B200MIX_ERR_UNSUPPORTED; }
         if(!(p.flags & B200MIX_VF_STOPPED))
         {
             if(p.flags & B200MIX_VF_STATIC)
@@ -1424,6 +1629,12 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
     {
         const b200mix_source_voice &p = voices[i];
         const bool stopped = (p.flags & B200MIX_VF_STOPPED) != 0;
+        // the voice no longer plays a callback buffer
+        if(!d->cbv.empty() && d->cbv[p.voice].slot >= 0)
+        {
+            d->cbv[p.voice].slot = -1;
+            --d->cb_bound;
+        }
         if(!d->h_send_slot.empty())
             for(uint32_t s2 = 0;s2 < B200MIX_MAX_SENDS;++s2)
             {
@@ -1601,7 +1812,7 @@ int b200mix_voice_queue(b200mix_device *d, uint32_t voice, uint32_t count, const
     Q.voice = voice; Q.count = count; Q.loop = loop_index;
     for(uint32_t i = 0;i < count;++i)
     {
-        if(buffers[i] >= dd.max_buffers || !d->h_buffers[buffers[i]].data)
+        if(buffers[i] >= dd.max_buffers || !d->h_buffers[buffers[i]].data || d->h_buffers[buffers[i]].pad)
         { d->error = "voice_queue: buffer id without data"; return B200MIX_ERR_INVALID; }
         Q.items[i] = buffers[i];
     }
@@ -1735,6 +1946,103 @@ static int run_bus_mix(b200mix_device *d, const SendMixParams &M, uint32_t num_e
 static inline void stage_mark(b200mix_device *d, int i)
 { if(d->profile_level >= 2) cudaEventRecord(d->ev_stage[i], d->stream); }
 
+// The callback buffers' part of an update (callback_plan.hpp).  First every callback buffer's
+// callbacks run on this thread; then, straight into the pinned arena, each buffer's plan record and
+// the blocks it has stored (ADPCM decoded to int16) are packed, its storage is compacted as the
+// reference does after the mix, and its voices' mirror advances; table and samples go to the GPU
+// with one copy on the mixer stream.  *plan stays null when no callback voice mixes this update.
+static int cb_plan_update(b200mix_device *d, uint32_t frames, const BufferRec *&plan)
+{
+    plan = nullptr;
+    if(int rc = cb_group(d)) { d->error = "render: " + d->error; return rc; }
+    const std::vector<int32_t> &reps = d->cb_reps;
+    bool any = false;
+    for(int32_t r : reps) any = any || r >= 0;
+    if(!any) return B200MIX_OK;
+    d->cb_work.resize(d->cbs.size());
+    // 1. the callbacks.  Registration guarantees the reference's storage size, which no request of
+    //    its chunk loop passes: plan_loads cannot stop half way through the buffers.
+    size_t size = align16(d->cbs.size()*sizeof(BufferRec));
+    for(size_t s = 0;s < d->cbs.size();++s)
+    {
+        if(reps[s] < 0) continue;
+        b200mix_device::CbBuf &c = d->cbs[s];
+        b200mix_device::CbWork &w = d->cb_work[s];
+        const b200mix_callback_buffer &cb = c.cb;
+        auto request = [&cb](uint64_t offset, uint32_t bytes) -> int64_t {
+            return cb.callback(cb.userptr, static_cast<char*>(cb.storage) + offset, int(bytes));
+        };
+        w.start = c.st;
+        if(!cbplan::plan_loads(c.st, cb.samples_per_block, cb.bytes_per_block, d->cbv[size_t(reps[s])].v,
+            frames, cb.storage_bytes, request, w.loads))
+        { d->error = "render: a callback request passes the callback buffer's storage"; return B200MIX_ERR_INVALID; }
+        // [pad | the stored blocks as the kernel reads them | pad], a pad holding one frame and
+        // 16 bytes: a load held at the last stored sample may address the frame before the first
+        // (none stored) or the first (empty span); the bulk copies round their runs up to 16 bytes
+        const size_t pad = align16(c.frame_bytes) + 16u;
+        w.bytes = w.loads.chunks ? size_t(c.st.num_blocks)*cb.samples_per_block*c.frame_bytes : 0u;
+        w.region = size + pad;
+        size = w.region + align16(w.bytes) + pad;
+    }
+    // 2. the arenas (the pinned one alternates: the other may still be in flight)
+    const int k = d->cb_idx;
+    if(d->cb_busy[k]) { CUDA_TRY(d, cudaEventSynchronize(d->cb_done[k])); d->cb_busy[k] = false; }
+    if(!d->cb_done[k]) CUDA_TRY(d, cudaEventCreateWithFlags(&d->cb_done[k], cudaEventDisableTiming));
+    if(size > d->h_cb_cap[k])
+    {
+        if(d->h_cb[k]) cudaFreeHost(d->h_cb[k]);
+        d->h_cb[k] = nullptr; d->h_cb_cap[k] = 0;
+        CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_cb[k]), size*2));
+        d->h_cb_cap[k] = size*2;
+    }
+    if(size > d->d_cb_cap)
+    {
+        CUDA_TRY(d, cudaStreamSynchronize(d->stream));     // the last update may still read it
+        cudaFree(d->d_cb);
+        d->d_cb = nullptr; d->d_cb_cap = 0;
+        CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_cb), size*2));
+        d->d_cb_cap = size*2;
+    }
+    // 3. pack, then what the reference does after the mix
+    uint8_t *arena = reinterpret_cast<uint8_t*>(d->h_cb[k]);
+    std::memset(arena, 0, size);
+    for(size_t s = 0;s < d->cbs.size();++s)
+    {
+        if(reps[s] < 0) continue;
+        b200mix_device::CbBuf &c = d->cbs[s];
+        const b200mix_device::CbWork &w = d->cb_work[s];
+        const b200mix_callback_buffer &cb = c.cb;
+        cbplan::Voice &vm = d->cbv[size_t(reps[s])].v;
+        const cbplan::Span span = cbplan::span_of(w.start, vm, cb.samples_per_block, c.st);
+        BufferRec rec = d->h_buffers[c.buffer];
+        rec.data = reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(d->d_cb)
+            + uintptr_t(int64_t(w.region) + span.base*int64_t(c.frame_bytes)));
+        rec.frames = w.loads.chunks ? span.frames : 0u;
+        std::memcpy(arena + s*sizeof(BufferRec), &rec, sizeof(rec));
+        uint8_t *dst = arena + w.region;
+        const uint8_t *src = static_cast<const uint8_t*>(cb.storage);
+        if(!w.bytes) {}
+        else if(cb.sample_type == B200MIX_FMT_IMA4)
+            DecodeIMA4(src, cb.channels, cb.samples_per_block, c.st.num_blocks, reinterpret_cast<int16_t*>(dst));
+        else if(cb.sample_type == B200MIX_FMT_MSADPCM)
+            DecodeMSADPCM(src, cb.channels, cb.samples_per_block, c.st.num_blocks, reinterpret_cast<int16_t*>(dst));
+        else
+            std::memcpy(dst, src, w.bytes);
+        const cbplan::After after = cbplan::finish_update(c.st, cb.samples_per_block, cb.bytes_per_block,
+            vm, frames);
+        if(after.consumed_bytes)
+            std::memmove(cb.storage, static_cast<char*>(cb.storage) + after.consumed_bytes, after.kept_bytes);
+        // the source's other channel voices move with it
+        for(uint32_t v : d->cb_members[s]) d->cbv[v].v = vm;
+    }
+    CUDA_TRY(d, cudaMemcpyAsync(d->d_cb, arena, size, cudaMemcpyHostToDevice, d->stream));
+    CUDA_TRY(d, cudaEventRecord(d->cb_done[k], d->stream));
+    d->cb_busy[k] = true;
+    d->cb_idx = k ^ 1;
+    plan = reinterpret_cast<const BufferRec*>(d->d_cb);
+    return B200MIX_OK;
+}
+
 // Phase A of an update: clear the mix buffers, mix every voice, reduce the partial rows and
 // finish the aux sends -> the slots' Wet buffers are complete (alc/alu.cpp:2196-2206).
 static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results, bool force_sends)
@@ -1747,6 +2055,10 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     if(dd.post_process == B200MIX_POST_AMBIDEC && !d->amb_in)
     { d->error = "render: ambisonic decoder not set"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
+    // callback buffers: their callbacks run here, before anything of the update is launched
+    const BufferRec *cbplan = nullptr;
+    if(d->cb_bound)
+        if(int rc = cb_plan_update(d, frames, cbplan)) return rc;
 
     stage_mark(d, 0);
     // clear MixBuffer (alc/alu.cpp:2417) and the wet buffers (alc/alu.cpp:2196-2198)
@@ -1815,6 +2127,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     P.qhdr = d->d_qhdr; P.queue = d->d_queue;
     P.claim = d->d_claim;
     P.dline = d->d_dline;
+    P.cbplan = cbplan;
     // the voice loop: resample (and park) -> direct filters -> deferred dry pass or HRIR FIR
     stage_mark(d, 1);
     if(d->profile) cudaEventRecord(d->ev_mix0, d->stream);

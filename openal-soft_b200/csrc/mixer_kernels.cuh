@@ -99,6 +99,14 @@ struct MixParams {
     // {count, head, loop, -} and kMaxQueue buffer ids
     uint4 *qhdr; const uint32_t *queue;
     uint32_t *claim;                         // {next order index, groups done}: zero between launches
+    // callback buffers (b200mix_buffer_callback): a BufferRec whose pad is 1 + s is read as
+    // cbplan[s] this update (null while no callback voice mixes; the record itself then reads
+    // as an empty buffer over zeros).  That record, planned on the
+    // host (callback_plan.hpp, Span), is the samples the buffer's callbacks delivered as a
+    // static buffer of `frames` frames that the voice's position addresses directly:
+    // LoadBufferCallback (core/voice.cpp:546-561) is then LoadBufferStatic without a loop, and
+    // the voice ends, as a static one, once its position reaches `frames` (core/voice.cpp:1158-1176).
+    const BufferRec *cbplan;
 };
 
 constexpr uint32_t kMaxQueue = 32, kNoLoop = 0xffffffffu;
@@ -1123,17 +1131,21 @@ k_mix_voices(const MixParams P)
         const uint32_t increment = h1.z;
         const uint32_t flags = h0.y;
         const bool haveBuffer = (flags & kVfHaveBuffer) != 0;
-        const BufferRec buf = P.buffers[haveBuffer ? h0.z : 0u];
+        // callback source (pad = 1 + its plan slot): the plan's record stands in for the buffer's,
+        // this update's span of the samples its callbacks delivered
+        const BufferRec rb = P.buffers[haveBuffer ? h0.z : 0u];
+        const BufferRec buf = (haveBuffer && rb.pad && P.cbplan) ? P.cbplan[rb.pad - 1u] : rb;
+        const uint32_t cbSlot = haveBuffer ? buf.pad : 0u;
         const uint32_t loopStart = h1.w, loopEnd = h2.x;
         int32_t intPos = int32_t(h1.x);
         uint32_t fracPos = h1.y;
-        bool looping = (flags & kVfLooping) != 0;
+        bool looping = (flags & kVfLooping) != 0 && cbSlot == 0u;
         if((flags & kVfStatic) && looping && haveBuffer && intPos >= 0
             && uint32_t(intPos) >= loopEnd)
             looping = false;                                     // core/voice.cpp:1015-1019
         const uint32_t resampler = h0.w;
         // streaming source (neither IsStatic nor callback): plays the voice's buffer queue
-        const bool isQueue = !(flags & kVfStatic) && P.qhdr != nullptr;
+        const bool isQueue = !(flags & kVfStatic) && P.qhdr != nullptr && cbSlot == 0u;
         const uint4 qh = isQueue ? P.qhdr[v] : make_uint4(0u, 0u, kNoLoop, 0u);
         const uint32_t *qitems = P.queue + size_t(v)*kMaxQueue;
         // mixed through its own HRIR by k_hrtf_fir (HRTF devices only)
@@ -1218,6 +1230,8 @@ k_mix_voices(const MixParams P)
             if(!defer)
                 mix_dry<GS, CDR>(accD, xs, S.newGain, P.dry_cur + size_t(v)*P.cd, P.dry_tgt + size_t(v)*P.cd,
                     P.cd, n, counter, playing, t);
+        // a callback voice's span ends where its stored samples do: the static end check is
+        // then the reference's (core/voice.cpp:1158-1176, see callback_plan.hpp)
         if(t == 0)
             write_back_voice(P, rec, v, h1, flags, vstate, increment, haveBuffer, isQueue, qh, qitems,
                 looping, loopStart, loopEnd, buf.frames);

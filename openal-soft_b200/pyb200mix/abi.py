@@ -56,6 +56,19 @@ class VoiceResult(C.Structure):
                 ("flags", C.c_uint32), ("buffers_done", C.c_uint32)]
 
 
+# b200mix_callback_fn (ALBUFFERCALLBACKTYPESOFT): int (*)(void *userptr, void *sampledata, int numbytes)
+CALLBACK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int)
+
+
+class CallbackBuffer(C.Structure):
+    """b200mix_callback_buffer (alBufferCallbackSOFT)."""
+    _fields_ = [("struct_size", C.c_uint32), ("sample_type", C.c_uint32), ("channels", C.c_uint32),
+                ("samples_per_block", C.c_uint32), ("bytes_per_block", C.c_uint32),
+                ("callback", CALLBACK_FN), ("userptr", C.c_void_p),
+                ("storage", C.c_void_p), ("storage_bytes", C.c_size_t),
+                ("num_blocks", C.c_uint32), ("block_offset", C.c_uint32), ("stopped", C.c_uint32)]
+
+
 class EfxReverb(C.Structure):
     """b200mix_efx_reverb (ReverbProps, core/effects/base.h:62-86)."""
     _fields_ = [("struct_size", C.c_uint32),
