@@ -30,16 +30,13 @@
 #include "hrtf_store.hpp"
 #include "adpcm.hpp"
 #include "callback_plan.hpp"
+#include "device_memory.hpp"
 
 using namespace b200mix;
 
 namespace {
 
 thread_local std::string g_create_error;
-
-struct DevBuf {           // cudaMalloc'ed array with size bookkeeping
-    void *ptr{nullptr}; size_t bytes{0};
-};
 
 } // namespace
 
@@ -53,101 +50,87 @@ struct b200mix_device {
 
     // tables
     BsincTable bsinc[3];
-    float *d_bsinc[3]{};
-    float *d_cubic[2]{};
+    DevArray<float> d_bsinc[3], d_cubic[2];
 
     // state
-    VoiceRec *d_voices{nullptr};
-    BufferRec *d_buffers{nullptr};
+    DevArray<VoiceRec> d_voices; DevArray<BufferRec> d_buffers;
     std::vector<BufferRec> h_buffers;
+    std::vector<DevArray<char>> buf_store;       // per buffer: the samples its h_buffers record views
     std::vector<uint32_t> h_vbuf;                 // static buffer an active voice plays (or NO_SLOT)
     std::vector<uint32_t> h_bufrefs;              // active static voices per buffer
-    float2 *d_hrtf_tgt{nullptr}, *d_hrtf_old{nullptr};
-    float *d_dry_cur{nullptr}, *d_dry_tgt{nullptr}, *d_send_cur{nullptr}, *d_send_tgt{nullptr};
+    DevArray<float2> d_hrtf_tgt, d_hrtf_old;
+    DevArray<float> d_dry_cur, d_dry_tgt, d_send_cur, d_send_tgt;
     VoiceResult *d_results{nullptr};              // inside d_outblock
     b200mix_voice_result *h_results{nullptr};     // inside h_outblock (pinned)
-    char *d_outblock{nullptr}, *h_outblock{nullptr}; size_t out_real_bytes{0};
+    DevArray<char> d_outblock; PinnedArray<char> h_outblock; size_t out_real_bytes{0};
 
     // mix buffers
     uint32_t dry_alloc_ch{0};
-    float *d_dry{nullptr}, *d_real{nullptr}, *d_wet{nullptr};
-    float *d_partial{nullptr}; size_t partial_floats{0};
-    float *d_accum_sum{nullptr};                  // [2][kAccumLen]
-    float *d_carry[2]{};                          // [2][kHrirLen] ping-pong
+    DevArray<float> d_dry, d_wet;
+    float *d_real{nullptr};                       // d_dry, or inside d_outblock
+    DevArray<float> d_partial; size_t partial_floats{0};
+    DevArray<float> d_accum_sum;                  // [2][kAccumLen]
+    DevArray<float> d_carry[2];                   // [2][kHrirLen] ping-pong
     int carry_idx{0};
     float *h_real{nullptr};                       // pinned [real][1024]
 
     // decoders
     uint32_t dec_channels{0}, dec_ir{0};
-    float2 *d_dec_coef{nullptr}; float *d_dec_hfscale{nullptr}, *d_dec_state{nullptr};
-    float *d_temp{nullptr}, *d_temp2{nullptr};
+    DevArray<float2> d_dec_coef; DevArray<float> d_dec_hfscale, d_dec_state;
+    DevArray<float> d_temp, d_temp2;
     uint32_t amb_in{0}; bool amb_dual{false};
-    float *d_amb_hf{nullptr}, *d_amb_lf{nullptr}, *d_amb_state{nullptr};
+    DevArray<float> d_amb_hf, d_amb_lf, d_amb_state;
     bool dry_active{false};
-    float *d_uhj_state{nullptr}, *d_uhj_scratch{nullptr};
+    DevArray<float> d_uhj_state, d_uhj_scratch;
     uint32_t stab_center{B200MIX_NO_SLOT};                // StablizerPostProcess: FrontCenter index
     float stab_coeff{0.0f};
-    float *d_stab_state{nullptr};                         // [0..2] MidFilter, [4+i] ChannelFilters[i].mApZ1
+    DevArray<float> d_stab_state;                         // [0..2] MidFilter, [4+i] ChannelFilters[i].mApZ1
     uint32_t bs2b_level{0};                               // Bs2bPostProcess: 0 = off
-    float *d_bs2b{nullptr};                               // [0..3] history, [4..8] coefficients
+    DevArray<float> d_bs2b;                               // [0..3] history, [4..8] coefficients
     uint32_t uhj_fir{0};                                  // 0 = IIR, 256 / 512 = UhjEncoder<N>
-    float *d_uhj_fir_state{nullptr}, *d_uhj_fir_coef{nullptr};
+    DevArray<float> d_uhj_fir_state, d_uhj_fir_coef;
 
-    // update staging (pinned host + device)
-    char *h_arena{nullptr}, *d_arena{nullptr};    // staging arena (see ensure_stage)
-    VoiceUpdate *h_upd{nullptr};                  // == h_arena
-    uint32_t stage_cap{0};
-    cudaEvent_t stage_done{nullptr};
-    bool stage_busy{false};
+    UploadArena stage;                            // b200mix_voices_update's inputs (see ensure_stage)
 
     // aux sends and effect slots
     std::vector<SlotRec> h_slots;            // host mirror (device pointers inside)
-    SlotRec *d_slots{nullptr};
-    std::vector<std::vector<void*>> slot_allocs;
+    DevArray<SlotRec> d_slots;
+    std::vector<std::vector<DevArray<char>>> slot_allocs;   // per slot: what its records point into
     uint32_t active_slots{0};
-    float *d_xscratch{nullptr};
-    uint32_t *d_sendinfo{nullptr};
+    DevArray<float> d_xscratch; DevArray<uint32_t> d_sendinfo;   // parked lines and state bits
     // direct/send filters (allocated by the first b200mix_voices_filters)
-    FilterRec *d_filt{nullptr};
-    FilterUpdate *h_fupd{nullptr}, *d_fupd{nullptr};
-    uint32_t fupd_cap{0};
-    cudaEvent_t fstage_done{nullptr};
-    bool fstage_busy{false};
-    float *d_fscratch{nullptr};
-    uint32_t fscratch_rows{0};
-    float *d_dline{nullptr};                 // [max_voices][1024] filtered direct-path lines
+    DevArray<FilterRec> d_filt;
+    UploadArena fstage;                      // b200mix_voices_filters' inputs
+    DevArray<float> d_fscratch, d_dline;     // [rows][1024]; [max_voices][1024] filtered direct-path lines
     std::vector<uint8_t> h_dfilt;            // host mirror: direct filter active per voice
     std::vector<uint32_t> h_order2;          // active voices with an active direct filter
-    uint32_t *d_order2{nullptr};
+    DevArray<uint32_t> d_order2;
     uint32_t num_order2{0};
     bool order2_dirty{false};
     std::vector<uint32_t> h_send_slot;       // [max_voices][MAX_SENDS] host mirror
     std::vector<uint32_t> h_slot_start;
     std::vector<SendEntry> h_entries;
-    uint32_t *d_slot_start{nullptr};
-    SendEntry *d_entries{nullptr};
+    DevArray<uint32_t> d_slot_start; DevArray<SendEntry> d_entries;
     uint32_t num_entries{0};
     bool sends_dirty{true};
     // EFX effect slots (b200mix_slot_efx): host mirrors + the per-slot views the kernel walks
-    struct EfxHost { bool used{false}; EfxParams p{}; EfxDev *dev{nullptr}; uint32_t mod_index{0}, mod_range{1};
+    struct EfxHost { bool used{false}; EfxParams p{}; DevArray<EfxDev> dev; uint32_t mod_index{0}, mod_range{1};
         uint32_t lfo_offset{0}, lfo_range{1}; };
     std::vector<EfxHost> efx;
-    EfxSlotView *d_efx_views{nullptr};
+    DevArray<EfxSlotView> d_efx_views;
     uint32_t efx_slots{0};
     uint32_t pshift_slots{0};                // EFX slots running the pitch shifter (k_efx_pshift)
     bool efx_ready{false};
-    float2 *d_twiddle{nullptr};
-    float *d_cubic_filter{nullptr};          // gCubicTable (reverb modulation taps)
+    DevArray<float2> d_twiddle; DevArray<float> d_cubic_filter;   // gCubicTable (reverb modulation taps)
     uint32_t reverb_slots{0};
 
     // attached HRTF data set (device-side HrtfStore::getCoeffs)
-    float2 *d_st_fields{nullptr}; uint2 *d_st_elevs{nullptr}; float2 *d_st_coeffs{nullptr};
-    uint8_t *d_st_delays{nullptr}; uint32_t st_num_fields{0}, st_ir{0};
-    uint4 *d_qhdr{nullptr}; uint32_t *d_queue{nullptr};   // streaming queues (first b200mix_voice_queue)
-    LimiterDev *d_limiter{nullptr};                      // DeviceBase::Limiter (b200mix_set_limiter)
-    float *d_limiter_delay{nullptr};                     // Compressor::mDelay [real_channels][1024]
-    uint32_t *d_dc_delay{nullptr}; float *d_dc_gain{nullptr}, *d_dc_buf{nullptr};   // DeviceBase::ChannelDelays
-    void *d_outbuf{nullptr}, *h_outbuf{nullptr};          // interleaved output staging (render_interleaved)
+    DevArray<float2> d_st_fields; DevArray<uint2> d_st_elevs; DevArray<float2> d_st_coeffs;
+    DevArray<uint8_t> d_st_delays; uint32_t st_num_fields{0}, st_ir{0};
+    DevArray<uint4> d_qhdr; DevArray<uint32_t> d_queue;   // streaming queues (ensure_queues)
+    DevArray<LimiterDev> d_limiter; DevArray<float> d_limiter_delay;   // DeviceBase::Limiter, Compressor::mDelay
+    DevArray<uint32_t> d_dc_delay; DevArray<float> d_dc_gain, d_dc_buf;   // DeviceBase::ChannelDelays
+    DevArray<char> d_outbuf; PinnedArray<char> h_outbuf;  // interleaved output staging (render_interleaved)
     // reverb slots: host side of ReverbState's two-pipeline state machine
     struct RvHost {
         bool used{false};
@@ -155,7 +138,7 @@ struct b200mix_device {
         uint32_t fade[2]{1u, 1u};               // mFadeSampleCount per pipeline object
         uint32_t offset{0};                     // mOffset
         ReverbDev h[2];                         // host mirrors (parameters + pointers)
-        ReverbDev *dev{nullptr};                // device array [2]
+        DevArray<ReverbDev> dev;                // device array [2]
     };
     std::vector<RvHost> rv;
     std::vector<uint32_t> h_target;          // EffectSlotBase::Target per slot (NO_SLOT = Dry)
@@ -166,49 +149,47 @@ struct b200mix_device {
     // parked dry bus (kernel variants without register dry accumulators)
     std::vector<uint8_t> h_hrtf;             // host mirror: voice mixes through its own HRIR
     std::vector<SendEntry> h_dry_entries;
-    SendEntry *d_dry_entries{nullptr};
-    uint32_t *d_dry_slot_start{nullptr};
+    DevArray<SendEntry> d_dry_entries; DevArray<uint32_t> d_dry_slot_start;
     uint32_t num_dry_entries{0};
     bool dry_entries_dirty{true};
-    float *d_dry_partial{nullptr};           // [kDryChunksMax][cd][1024]
-    float *d_dry_geff{nullptr};              // [max_voices][cd]
-    float *d_send_geff{nullptr};             // [max_voices*num_sends][cw]
-    float4 *d_dry_gramp{nullptr}, *d_send_gramp{nullptr};
-    float *d_send_partial{nullptr};          // [send_chunks][max_slots][cw][1024]
-    uint32_t send_partial_chunks{0}, max_slot_entries{0};
+    DevArray<float> d_dry_partial;           // [kDryChunksMax][cd][1024]
+    DevArray<float> d_dry_geff;              // [max_voices][cd]
+    DevArray<float> d_send_geff;             // [max_voices*num_sends][cw]
+    DevArray<float4> d_dry_gramp, d_send_gramp;
+    DevArray<float> d_send_partial;          // [send_chunks][max_slots][cw][1024]
+    uint32_t max_slot_entries{0};
     bool profile{false};
-    cudaEvent_t ev_mix0{nullptr}, ev_mix1{nullptr};
+    Event ev_mix0, ev_mix1;
     bool ev_valid{false};
     // stage marks of the last update (profile >= 2): see b200mix_last_stage_ms
     static constexpr int kStages = 8;
-    cudaEvent_t ev_stage[kStages + 1]{};
+    Event ev_stage[kStages + 1];
     bool stage_valid{false}; int profile_level{0};
 
     // mixing order (host mirror of which voices are configured active, and their cost)
     std::vector<uint8_t> h_active;
     std::vector<uint32_t> h_cost;
     std::vector<uint32_t> h_order;
-    uint32_t *d_order{nullptr};
+    DevArray<uint32_t> d_order;
     uint32_t num_order{0};
     bool order_dirty{true};
 
     // GPU parameter stage (b200mix_sources_update): pinned input staging + device scratch
-    char *h_src{nullptr}, *d_src{nullptr}; uint32_t src_cap{0};
-    cudaEvent_t src_done{nullptr}; bool src_busy{false};
+    UploadArena src;
     bool dev_filters{false};                 // filter activity is decided on the device: order2 = order
     bool panmix_tc{false};                   // wide dry buses: pan-mix past the fades on the tensor cores
 
     // voice-sharded device set (b200mix_shard_*): transport 0 none, 1 peer stores, 2 NCCL
     struct Shard {
         uint32_t rank{0}, world{1}; int transport{0};
-        char *own{nullptr}; size_t bytes{0};
+        DevArray<char> own;
         char *peer[kShardMaxWorld]{};
         size_t off_real{0}, off_wet{0}, real_floats{0}, wet_src_floats{0};
         uint32_t owned_max{0};
         uint32_t epoch{0};
-        uint32_t *d_counters{nullptr};         // [0] real push, [1] real sum, [2] wet sum, [4..] wet push per owner
-        uint32_t *h_status{nullptr};           // pinned copy of ShardCtl::status
-        cudaEvent_t ev[4]{};                   // wet exchange begin/end, RealOut reduce begin/end
+        DevArray<uint32_t> d_counters;         // [0] real push, [1] real sum, [2] wet sum, [4..] wet push per owner
+        PinnedArray<uint32_t> h_status;        // pinned copy of ShardCtl::status
+        Event ev[4];                           // wet exchange begin/end, RealOut reduce begin/end
         bool ev_wet{false}, ev_real{false};
         // NCCL transport (dlopen'ed: the library carries no link-time NCCL dependency)
         void *nccl_lib{nullptr}; void *comm{nullptr};
@@ -223,7 +204,7 @@ struct b200mix_device {
     void (*mix_fn)(const MixParams){nullptr};
     size_t mix_smem{0}; int mix_cdr{0}; int mix_blocks_per_sm{1};
     uint32_t reverb_seq{0};          // update counter of k_reverb_process' early/late hand-off (24 bits used)
-    uint32_t *d_claim{nullptr};      // voice claim counters of the parking k_mix_voices
+    DevArray<uint32_t> d_claim;      // voice claim counters of the parking k_mix_voices
     int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
 
     // callback buffers (b200mix_buffer_callback): the registrations (plan slots), the host's
@@ -242,13 +223,13 @@ struct b200mix_device {
     struct CbVoice { int32_t slot{-1}; cbplan::Voice v{}; };
     std::vector<CbVoice> cbv;                // per voice
     uint32_t cb_bound{0};                    // voices bound to a callback buffer
-    char *h_cb[2]{}; size_t h_cb_cap[2]{}; cudaEvent_t cb_done[2]{}; bool cb_busy[2]{}; int cb_idx{0};
-    char *d_cb{nullptr}; size_t d_cb_cap{0};
-    void *d_cb_zero{nullptr};                // zeros behind every callback buffer's own record
+    UploadArena cb_arena[2]; int cb_idx{0};
+    DevArray<char> d_cb_zero;                // zeros behind every callback buffer's own record
     std::vector<int32_t> cb_reps;            // per slot: the voice the update is planned from (-1: none)
     std::vector<std::vector<uint32_t>> cb_members;   // per slot: its other mixing voices
     struct CbWork { cbplan::State start; cbplan::Loads loads; size_t region{0}, bytes{0}; };
     std::vector<CbWork> cb_work;             // per slot, for the update being planned
+    ~b200mix_device() { if(stream) cudaStreamDestroy(stream); }
 };
 
 namespace {
@@ -261,13 +242,14 @@ namespace {
 #define CUDA_TRY(dev, expr) do { cudaError_t e_ = (expr); if(e_ != cudaSuccess) {            \
     (dev)->error = std::string(#expr) + ": " + cudaGetErrorString(e_); return B200MIX_ERR_CUDA; } } while(0)
 
+// Copies a host vector to the front of a device array, then synchronises the stream: the vector
+// may be rebuilt (or go away) before an asynchronous copy would have read it.
 template<typename T>
-int dev_alloc(b200mix_device *d, T *&p, size_t count, bool zero = true)
+int upload(b200mix_device *d, DevArray<T> &dst, const std::vector<T> &src)
 {
-    p = nullptr;
-    if(count == 0) return B200MIX_OK;
-    CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&p), count*sizeof(T)));
-    if(zero) CUDA_TRY(d, cudaMemsetAsync(p, 0, count*sizeof(T), d->stream));
+    if(!src.empty())
+        CUDA_TRY(d, cudaMemcpyAsync(dst.get(), src.data(), src.size()*sizeof(T), cudaMemcpyHostToDevice, d->stream));
+    CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     return B200MIX_OK;
 }
 
@@ -285,16 +267,27 @@ FirVariant get_fir(uint32_t ir_size)
 
 constexpr uint32_t kDryChunksMax = 128;
 
+// The parts allocated on first use below go into locals and move into the device only once all
+// succeeded: a failure leaves the device as it was, and the call can be retried.
+// Parked lines and state bits of every voice: the parking k_mix_voices writes them, the sends,
+// the direct filters and the parked dry bus read them.
+int ensure_park_lines(b200mix_device *d)
+{
+    if(d->d_xscratch) return B200MIX_OK;
+    const uint32_t nv = d->desc.max_voices;
+    DevArray<float> xscratch; DevArray<uint32_t> sendinfo;
+    CUDA_TRY(d, xscratch.alloc(size_t(nv)*kLine, d->stream));
+    CUDA_TRY(d, sendinfo.alloc(nv, d->stream));
+    d->d_xscratch = std::move(xscratch); d->d_sendinfo = std::move(sendinfo);
+    return B200MIX_OK;
+}
+
 // Storage of the parked dry bus (variants with CDR == 0 that meet a non-HRTF voice).
 int ensure_dry_park(b200mix_device *d)
 {
     const b200mix_device_desc &dd = d->desc;
     if(d->d_dry_entries) return B200MIX_OK;
-    if(!d->d_xscratch)
-        if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
-    if(!d->d_sendinfo)
-        if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
-    if(int rc = dev_alloc(d, d->d_dry_entries, dd.max_voices)) return rc;
+    if(int rc = ensure_park_lines(d)) return rc;
     if(dd.dry_channels > 4u && dd.dry_channels <= uint32_t(kPmN))
     {
         CUDA_TRY(d, cudaFuncSetAttribute(k_panmix_tc, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -303,37 +296,54 @@ int ensure_dry_park(b200mix_device *d)
         const char *simt = std::getenv("B200MIX_PANMIX_SIMT");
         d->panmix_tc = !(simt && simt[0] == '1');
     }
-    if(int rc = dev_alloc(d, d->d_dry_slot_start, 2)) return rc;
-    if(int rc = dev_alloc(d, d->d_dry_partial, size_t(kDryChunksMax)*dd.dry_channels*kLine)) return rc;
-    if(int rc = dev_alloc(d, d->d_dry_geff, size_t(dd.max_voices)*dd.dry_channels)) return rc;
-    if(int rc = dev_alloc(d, d->d_dry_gramp, size_t(dd.max_voices)*dd.dry_channels)) return rc;
+    DevArray<SendEntry> entries; DevArray<uint32_t> slotStart;
+    DevArray<float> partial, geff; DevArray<float4> gramp;
+    CUDA_TRY(d, entries.alloc(dd.max_voices, d->stream));
+    CUDA_TRY(d, slotStart.alloc(2, d->stream));
+    CUDA_TRY(d, partial.alloc(size_t(kDryChunksMax)*dd.dry_channels*kLine, d->stream));
+    CUDA_TRY(d, geff.alloc(size_t(dd.max_voices)*dd.dry_channels, d->stream));
+    CUDA_TRY(d, gramp.alloc(size_t(dd.max_voices)*dd.dry_channels, d->stream));
+    d->d_dry_entries = std::move(entries); d->d_dry_slot_start = std::move(slotStart);
+    d->d_dry_partial = std::move(partial); d->d_dry_geff = std::move(geff); d->d_dry_gramp = std::move(gramp);
     return B200MIX_OK;
 }
 
-// One pinned + one device staging arena for b200mix_voices_update: a call packs
-// [VoiceUpdate n][coefficients or directions][dry gains][send gains] back to back (16-byte
-// aligned parts) and ships them with ONE host-to-device copy.
-static size_t align16(size_t v) { return (v + 15u) & ~size_t(15); }
+// Queue tables of the streaming voices (the first voice that reads a queue).
+int ensure_queues(b200mix_device *d)
+{
+    if(d->d_qhdr) return B200MIX_OK;
+    const uint32_t nv = d->desc.max_voices;
+    DevArray<uint4> qhdr; DevArray<uint32_t> queue;
+    CUDA_TRY(d, qhdr.alloc(nv, d->stream));
+    CUDA_TRY(d, queue.alloc(size_t(nv)*kMaxQueue, d->stream));
+    d->d_qhdr = std::move(qhdr); d->d_queue = std::move(queue);
+    return B200MIX_OK;
+}
 
+// `count` zeroed T for the records of `slot`; the slot owns them until free_slot.
+template<typename T>
+int slot_alloc(b200mix_device *d, uint32_t slot, T *&p, size_t count)
+{
+    DevArray<char> a;
+    CUDA_TRY(d, a.alloc(count*sizeof(T), d->stream));
+    p = reinterpret_cast<T*>(a.get());
+    d->slot_allocs[slot].push_back(std::move(a));
+    return B200MIX_OK;
+}
+
+static size_t align16(size_t v) { return UploadArena::align(v); }
+
+// b200mix_voices_update's arena: a call packs [VoiceUpdate n][coefficients or directions]
+// [dry gains][send gains] and ships them with one copy.  It holds at least 256 voices.
 int ensure_stage(b200mix_device *d, uint32_t n)
 {
-    if(n <= d->stage_cap) return B200MIX_OK;
     const b200mix_device_desc &dd = d->desc;
-    if(d->stage_cap)
-    {
-        cudaStreamSynchronize(d->stream);
-        cudaFreeHost(d->h_arena); cudaFree(d->d_arena);
-        d->h_arena = nullptr; d->d_arena = nullptr;
-    }
     const uint32_t cap = std::max<uint32_t>(n, 256u);
     const size_t bytes = align16(size_t(cap)*sizeof(VoiceUpdate))
         + align16(size_t(cap)*std::max<size_t>(size_t(dd.ir_size)*2, 4)*sizeof(float))
         + align16(size_t(cap)*dd.dry_channels*sizeof(float))
         + align16(size_t(cap)*dd.num_sends*dd.wet_channels*sizeof(float)) + 64;
-    CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_arena), bytes));
-    CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_arena), bytes));
-    d->h_upd = reinterpret_cast<VoiceUpdate*>(d->h_arena);
-    d->stage_cap = cap;
+    CUDA_TRY(d, d->stage.reserve(n, cap, bytes, bytes, d->stream));
     return B200MIX_OK;
 }
 
@@ -390,8 +400,6 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
     d->num_sms = prop.multiProcessorCount;
     if(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking) != cudaSuccess)
     { d->error = "cudaStreamCreate failed"; return fail(B200MIX_ERR_CUDA); }
-    if(cudaEventCreateWithFlags(&d->stage_done, cudaEventDisableTiming) != cudaSuccess)
-    { d->error = "cudaEventCreate failed"; return fail(B200MIX_ERR_CUDA); }
 
     auto run = [&]() -> int {
         // resampler tables (core/bsinc_tables.cpp:150-155)
@@ -400,40 +408,38 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         d->bsinc[2] = BuildBsincTable(80, 47, 1);
         for(int i = 0;i < 3;++i)
         {
-            if(int rc = dev_alloc(d, d->d_bsinc[i], d->bsinc[i].tab.size(), false)) return rc;
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_bsinc[i], d->bsinc[i].tab.data(),
-                d->bsinc[i].tab.size()*sizeof(float), cudaMemcpyHostToDevice, d->stream));
+            CUDA_TRY(d, d->d_bsinc[i].alloc(d->bsinc[i].tab.size()));
+            if(int rc = upload(d, d->d_bsinc[i], d->bsinc[i].tab)) return rc;
         }
         const std::vector<float> cubic[2] = {BuildSplineTable(), BuildGaussianTable()};
         for(int i = 0;i < 2;++i)
         {
-            if(int rc = dev_alloc(d, d->d_cubic[i], cubic[i].size(), false)) return rc;
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_cubic[i], cubic[i].data(), cubic[i].size()*sizeof(float),
-                cudaMemcpyHostToDevice, d->stream));
+            CUDA_TRY(d, d->d_cubic[i].alloc(cubic[i].size()));
+            if(int rc = upload(d, d->d_cubic[i], cubic[i])) return rc;
         }
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));   // cubic[] goes out of scope
 
         const b200mix_device_desc &dd = d->desc;
         d->ir_pad = (dd.ir_size + 7u) & ~7u;
-        if(int rc = dev_alloc(d, d->d_voices, dd.max_voices)) return rc;
-        if(int rc = dev_alloc(d, d->d_buffers, std::max(dd.max_buffers, 1u))) return rc;
+        CUDA_TRY(d, d->d_voices.alloc(dd.max_voices, d->stream));
+        CUDA_TRY(d, d->d_buffers.alloc(std::max(dd.max_buffers, 1u), d->stream));
         d->h_buffers.assign(std::max(dd.max_buffers, 1u), BufferRec{});
+        d->buf_store.resize(d->h_buffers.size());
         d->h_vbuf.assign(dd.max_voices, B200MIX_NO_SLOT);
         d->h_bufrefs.assign(std::max(dd.max_buffers, 1u), 0u);
         if(dd.ir_size)
         {
-            if(int rc = dev_alloc(d, d->d_hrtf_tgt, size_t(dd.max_voices)*d->ir_pad)) return rc;
-            if(int rc = dev_alloc(d, d->d_hrtf_old, size_t(dd.max_voices)*d->ir_pad)) return rc;
+            CUDA_TRY(d, d->d_hrtf_tgt.alloc(size_t(dd.max_voices)*d->ir_pad, d->stream));
+            CUDA_TRY(d, d->d_hrtf_old.alloc(size_t(dd.max_voices)*d->ir_pad, d->stream));
         }
-        if(int rc = dev_alloc(d, d->d_dry_cur, size_t(dd.max_voices)*std::max(dd.dry_channels, 1u))) return rc;
-        if(int rc = dev_alloc(d, d->d_dry_tgt, size_t(dd.max_voices)*std::max(dd.dry_channels, 1u))) return rc;
+        CUDA_TRY(d, d->d_dry_cur.alloc(size_t(dd.max_voices)*std::max(dd.dry_channels, 1u), d->stream));
+        CUDA_TRY(d, d->d_dry_tgt.alloc(size_t(dd.max_voices)*std::max(dd.dry_channels, 1u), d->stream));
         if(dd.num_sends && dd.wet_channels)
         {
             const size_t per = size_t(dd.num_sends)*dd.wet_channels;
-            if(int rc = dev_alloc(d, d->d_send_cur, dd.max_voices*per)) return rc;
-            if(int rc = dev_alloc(d, d->d_send_tgt, dd.max_voices*per)) return rc;
+            CUDA_TRY(d, d->d_send_cur.alloc(dd.max_voices*per, d->stream));
+            CUDA_TRY(d, d->d_send_tgt.alloc(dd.max_voices*per, d->stream));
         }
-        if(int rc = dev_alloc(d, d->d_order, dd.max_voices)) return rc;
+        CUDA_TRY(d, d->d_order.alloc(dd.max_voices, d->stream));
         d->h_active.assign(dd.max_voices, 0);
         d->h_cost.assign(dd.max_voices, 0);
         d->h_hrtf.assign(dd.max_voices, 0);
@@ -462,9 +468,8 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         if(d->mix_cdr == 0)
         {
             // the parking variant writes every mixed voice's line and state bits
-            if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
-            if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
-            if(int rc = dev_alloc(d, d->d_claim, 2)) return rc;
+            if(int rc = ensure_park_lines(d)) return rc;
+            CUDA_TRY(d, d->d_claim.alloc(2, d->stream));
         }
         if(hrtfDev)
         {
@@ -477,50 +482,46 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         }
 
         d->dry_alloc_ch = std::max<uint32_t>(std::max(dd.dry_channels, 1u), uint32_t(d->mix_cdr));
-        if(int rc = dev_alloc(d, d->d_dry, size_t(d->dry_alloc_ch)*kLine)) return rc;
+        CUDA_TRY(d, d->d_dry.alloc(size_t(d->dry_alloc_ch)*kLine, d->stream));
         // RealOut and the voice results share one block (and one pinned mirror): a render that
         // returns both needs ONE device-to-host copy
         {
             const size_t realFloats = size_t(std::max(dd.real_channels, 1u))*kLine;
             static_assert(sizeof(VoiceResult) == 16 && sizeof(b200mix_voice_result) == 16, "result layout");
             const size_t blockBytes = realFloats*sizeof(float) + size_t(dd.max_voices)*sizeof(VoiceResult);
-            char *blk = nullptr;
-            if(int rc = dev_alloc(d, blk, blockBytes)) return rc;
-            d->d_outblock = blk;
+            CUDA_TRY(d, d->d_outblock.alloc(blockBytes, d->stream));
+            char *blk = d->d_outblock;
             d->d_results = reinterpret_cast<VoiceResult*>(blk + realFloats*sizeof(float));
-            CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_outblock), blockBytes));
-            d->h_real = reinterpret_cast<float*>(d->h_outblock);
+            CUDA_TRY(d, d->h_outblock.alloc(blockBytes));
+            d->h_real = reinterpret_cast<float*>(d->h_outblock.get());
             d->h_results = reinterpret_cast<b200mix_voice_result*>(d->h_outblock + realFloats*sizeof(float));
             d->out_real_bytes = realFloats*sizeof(float);
             if(dd.post_process == B200MIX_POST_NONE) d->d_real = d->d_dry;
             else d->d_real = reinterpret_cast<float*>(blk);
         }
         if(dd.max_slots && dd.wet_channels)
-            if(int rc = dev_alloc(d, d->d_wet, size_t(dd.max_slots)*dd.wet_channels*kLine)) return rc;
+            CUDA_TRY(d, d->d_wet.alloc(size_t(dd.max_slots)*dd.wet_channels*kLine, d->stream));
         // partial rows: the FIR's HrtfAccumData rows (HRTF devices), or the register dry bus'
         // rows in two regions, k_mix_voices' and k_mix_deferred's (voices with direct filters)
         d->partial_floats = hrtfDev ? size_t(d->num_sms)*d->fir_blocks_per_sm*(2*kAccumLen)
             : size_t(d->num_sms)*d->mix_blocks_per_sm*size_t(d->mix_cdr)*kLine;
-        if(int rc = dev_alloc(d, d->d_partial, std::max<size_t>((hrtfDev ? 1 : 2)*d->partial_floats, 4))) return rc;
-        if(int rc = dev_alloc(d, d->d_accum_sum, 2*kAccumLen)) return rc;
-        if(int rc = dev_alloc(d, d->d_carry[0], 2*kHrirLen)) return rc;
-        if(int rc = dev_alloc(d, d->d_carry[1], 2*kHrirLen)) return rc;
-        if(int rc = dev_alloc(d, d->d_temp, size_t(std::max(dd.dry_channels, 1u))*kLine)) return rc;
-        if(int rc = dev_alloc(d, d->d_temp2, size_t(std::max(dd.dry_channels, 1u))*kLine)) return rc;
+        CUDA_TRY(d, d->d_partial.alloc(std::max<size_t>((hrtfDev ? 1 : 2)*d->partial_floats, 4), d->stream));
+        CUDA_TRY(d, d->d_accum_sum.alloc(2*kAccumLen, d->stream));
+        CUDA_TRY(d, d->d_carry[0].alloc(2*kHrirLen, d->stream));
+        CUDA_TRY(d, d->d_carry[1].alloc(2*kHrirLen, d->stream));
+        CUDA_TRY(d, d->d_temp.alloc(size_t(std::max(dd.dry_channels, 1u))*kLine, d->stream));
+        CUDA_TRY(d, d->d_temp2.alloc(size_t(std::max(dd.dry_channels, 1u))*kLine, d->stream));
         if(dd.max_slots && dd.wet_channels && dd.num_sends)
         {
             d->h_slots.assign(dd.max_slots, SlotRec{});
-            d->slot_allocs.assign(dd.max_slots, {});
-            if(int rc = dev_alloc(d, d->d_slots, dd.max_slots)) return rc;
-            if(!d->d_xscratch)
-                if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
-            if(!d->d_sendinfo)
-                if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
-            if(int rc = dev_alloc(d, d->d_send_geff, size_t(dd.max_voices)*dd.num_sends*dd.wet_channels)) return rc;
-            if(int rc = dev_alloc(d, d->d_send_gramp, size_t(dd.max_voices)*dd.num_sends*dd.wet_channels)) return rc;
+            d->slot_allocs.resize(dd.max_slots);
+            CUDA_TRY(d, d->d_slots.alloc(dd.max_slots, d->stream));
+            if(int rc = ensure_park_lines(d)) return rc;
+            CUDA_TRY(d, d->d_send_geff.alloc(size_t(dd.max_voices)*dd.num_sends*dd.wet_channels, d->stream));
+            CUDA_TRY(d, d->d_send_gramp.alloc(size_t(dd.max_voices)*dd.num_sends*dd.wet_channels, d->stream));
             d->h_send_slot.assign(size_t(dd.max_voices)*B200MIX_MAX_SENDS, B200MIX_NO_SLOT);
-            if(int rc = dev_alloc(d, d->d_slot_start, dd.max_slots + 1)) return rc;
-            if(int rc = dev_alloc(d, d->d_entries, size_t(dd.max_voices)*dd.num_sends)) return rc;
+            CUDA_TRY(d, d->d_slot_start.alloc(dd.max_slots + 1, d->stream));
+            CUDA_TRY(d, d->d_entries.alloc(size_t(dd.max_voices)*dd.num_sends, d->stream));
             std::vector<float2> tw(128);
             for(int k = 0;k < 128;++k)
             {
@@ -528,19 +529,15 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
                 tw[k] = make_float2(float(std::cos(a)), float(std::sin(a)));
             }
             const std::vector<float> cf = BuildCubicFilter();
-            if(int rc = dev_alloc(d, d->d_cubic_filter, cf.size(), false)) return rc;
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_cubic_filter, cf.data(), cf.size()*sizeof(float),
-                cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-            if(int rc = dev_alloc(d, d->d_twiddle, 128, false)) return rc;
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_twiddle, tw.data(), 128*sizeof(float2),
-                cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            CUDA_TRY(d, d->d_cubic_filter.alloc(cf.size()));
+            if(int rc = upload(d, d->d_cubic_filter, cf)) return rc;
+            CUDA_TRY(d, d->d_twiddle.alloc(tw.size()));
+            if(int rc = upload(d, d->d_twiddle, tw)) return rc;
         }
         if(dd.post_process == B200MIX_POST_UHJ || dd.post_process == B200MIX_POST_TSME)
         {
-            if(int rc = dev_alloc(d, d->d_uhj_state, 64)) return rc;
-            if(int rc = dev_alloc(d, d->d_uhj_scratch, 5*1025)) return rc;
+            CUDA_TRY(d, d->d_uhj_state.alloc(64, d->stream));
+            CUDA_TRY(d, d->d_uhj_scratch.alloc(5*1025, d->stream));
         }
         if(int rc = ensure_stage(d, std::min(dd.max_voices, 4096u))) return rc;
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
@@ -557,52 +554,12 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
 void b200mix_destroy(b200mix_device *d)
 {
     if(!d) return;
-    if(d->stream) cudaStreamSynchronize(d->stream);
-    shard_release(d);
-    for(auto &b : d->h_buffers) if(b.data && !b.pad) cudaFree(const_cast<void*>(b.data));
-    cudaFree(d->d_cb_zero);
-    for(int i = 0;i < 3;++i) cudaFree(d->d_bsinc[i]);
-    for(int i = 0;i < 2;++i) cudaFree(d->d_cubic[i]);
-    cudaFree(d->d_voices); cudaFree(d->d_buffers); cudaFree(d->d_hrtf_tgt); cudaFree(d->d_hrtf_old);
-    cudaFree(d->d_dry_cur); cudaFree(d->d_dry_tgt); cudaFree(d->d_send_cur); cudaFree(d->d_send_tgt);
-    cudaFree(d->d_outblock); cudaFreeHost(d->h_outblock); cudaFree(d->d_order);
-    cudaFree(d->d_dry); cudaFree(d->d_wet); cudaFree(d->d_partial); cudaFree(d->d_accum_sum);
-    cudaFree(d->d_carry[0]); cudaFree(d->d_carry[1]);
-    cudaFree(d->d_dec_coef); cudaFree(d->d_dec_hfscale); cudaFree(d->d_dec_state);
-    cudaFree(d->d_temp); cudaFree(d->d_temp2);
-    cudaFree(d->d_amb_hf); cudaFree(d->d_amb_lf); cudaFree(d->d_amb_state);
-    cudaFree(d->d_uhj_state); cudaFree(d->d_uhj_scratch);
-    cudaFree(d->d_uhj_fir_state); cudaFree(d->d_uhj_fir_coef); cudaFree(d->d_bs2b); cudaFree(d->d_stab_state);
-    for(auto &v : d->slot_allocs) for(void *p : v) cudaFree(p);
-    cudaFree(d->d_slots); cudaFree(d->d_xscratch); cudaFree(d->d_sendinfo); cudaFree(d->d_claim);
-    cudaFree(d->d_filt); cudaFree(d->d_fupd); cudaFree(d->d_fscratch);
-    cudaFree(d->d_dline); cudaFree(d->d_order2); cudaFree(d->d_qhdr); cudaFree(d->d_queue);
-    cudaFree(d->d_outbuf); if(d->h_outbuf) cudaFreeHost(d->h_outbuf);
-    cudaFree(d->d_limiter); cudaFree(d->d_limiter_delay);
-    cudaFree(d->d_dc_delay); cudaFree(d->d_dc_gain); cudaFree(d->d_dc_buf);
-    cudaFree(d->d_st_fields); cudaFree(d->d_st_elevs); cudaFree(d->d_st_coeffs); cudaFree(d->d_st_delays);
-    cudaFree(d->d_dry_entries); cudaFree(d->d_dry_slot_start); cudaFree(d->d_dry_partial);
-    cudaFree(d->d_dry_geff); cudaFree(d->d_send_geff); cudaFree(d->d_send_partial);
-    cudaFree(d->d_dry_gramp); cudaFree(d->d_send_gramp);
-    if(d->h_fupd) cudaFreeHost(d->h_fupd);
-    if(d->fstage_done) cudaEventDestroy(d->fstage_done);
-    cudaFree(d->d_slot_start); cudaFree(d->d_entries); cudaFree(d->d_twiddle); cudaFree(d->d_cubic_filter);
-    cudaFree(d->d_efx_views);
-    cudaFreeHost(d->h_arena); cudaFree(d->d_arena);
-    if(d->h_src) cudaFreeHost(d->h_src);
-    cudaFree(d->d_src);
-    if(d->src_done) cudaEventDestroy(d->src_done);
-    if(d->stage_done) cudaEventDestroy(d->stage_done);
-    for(int i = 0;i < 2;++i)
+    if(d->stream)
     {
-        if(d->h_cb[i]) cudaFreeHost(d->h_cb[i]);
-        if(d->cb_done[i]) cudaEventDestroy(d->cb_done[i]);
+        cudaSetDevice(d->cuda_dev);
+        cudaStreamSynchronize(d->stream);
     }
-    cudaFree(d->d_cb);
-    if(d->ev_mix0) cudaEventDestroy(d->ev_mix0);
-    if(d->ev_mix1) cudaEventDestroy(d->ev_mix1);
-    for(cudaEvent_t e : d->ev_stage) if(e) cudaEventDestroy(e);
-    if(d->stream) cudaStreamDestroy(d->stream);
+    shard_release(d);
     delete d;
 }
 
@@ -613,11 +570,10 @@ int b200mix_set_hrtf_decoder(b200mix_device *d, uint32_t channels, uint32_t ir_s
         || !hf_scale || !splitter_coeff || d->desc.post_process != B200MIX_POST_HRTF)
     { if(d) d->error = "set_hrtf_decoder: bad arguments"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    cudaFree(d->d_dec_coef); cudaFree(d->d_dec_hfscale); cudaFree(d->d_dec_state);
     d->dec_channels = channels; d->dec_ir = ir_size;
-    if(int rc = dev_alloc(d, d->d_dec_coef, size_t(channels)*ir_size, false)) return rc;
-    if(int rc = dev_alloc(d, d->d_dec_hfscale, channels, false)) return rc;
-    if(int rc = dev_alloc(d, d->d_dec_state, size_t(channels)*4)) return rc;
+    CUDA_TRY(d, d->d_dec_coef.alloc(size_t(channels)*ir_size));
+    CUDA_TRY(d, d->d_dec_hfscale.alloc(channels));
+    CUDA_TRY(d, d->d_dec_state.alloc(size_t(channels)*4));
     std::vector<float> st(size_t(channels)*4, 0.0f);
     for(uint32_t c = 0;c < channels;++c) st[c*4] = splitter_coeff[c];
     CUDA_TRY(d, cudaMemcpyAsync(d->d_dec_coef, coeffs, size_t(channels)*ir_size*2*sizeof(float),
@@ -637,20 +593,19 @@ int b200mix_set_ambi_decoder(b200mix_device *d, uint32_t in_channels, const floa
         || d->desc.post_process != B200MIX_POST_AMBIDEC)
     { if(d) d->error = "set_ambi_decoder: bad arguments"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    cudaFree(d->d_amb_hf); cudaFree(d->d_amb_lf); cudaFree(d->d_amb_state);
-    d->d_amb_lf = nullptr;
+    d->d_amb_lf.reset();
     const size_t n = size_t(in_channels)*d->desc.real_channels;
     d->amb_in = in_channels; d->amb_dual = gains_lf != nullptr;
-    if(int rc = dev_alloc(d, d->d_amb_hf, n, false)) return rc;
+    CUDA_TRY(d, d->d_amb_hf.alloc(n));
     CUDA_TRY(d, cudaMemcpyAsync(d->d_amb_hf, gains_hf, n*sizeof(float), cudaMemcpyHostToDevice, d->stream));
     if(gains_lf)
     {
-        if(int rc = dev_alloc(d, d->d_amb_lf, n, false)) return rc;
+        CUDA_TRY(d, d->d_amb_lf.alloc(n));
         CUDA_TRY(d, cudaMemcpyAsync(d->d_amb_lf, gains_lf, n*sizeof(float), cudaMemcpyHostToDevice, d->stream));
     }
     std::vector<float> st(size_t(in_channels)*4, 0.0f);
     for(uint32_t c = 0;c < in_channels;++c) st[c*4] = xover_coeff;
-    if(int rc = dev_alloc(d, d->d_amb_state, st.size(), false)) return rc;
+    CUDA_TRY(d, d->d_amb_state.alloc(st.size()));
     CUDA_TRY(d, cudaMemcpyAsync(d->d_amb_state, st.data(), st.size()*sizeof(float),
         cudaMemcpyHostToDevice, d->stream));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
@@ -710,7 +665,7 @@ int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_ca
     { d->error = "buffer_callback: state outside the storage"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     if(!d->d_cb_zero)
-        if(int rc = dev_alloc(d, d->d_cb_zero, kCbPad)) return rc;
+        CUDA_TRY(d, d->d_cb_zero.alloc(kCbPad, d->stream));
     if(d->cb_of_buffer.empty())
     {
         d->cb_of_buffer.assign(dd.max_buffers, -1);
@@ -725,7 +680,7 @@ int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_ca
         if(h.data)
         {
             CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-            cudaFree(const_cast<void*>(h.data));
+            d->buf_store[buffer].reset();
         }
         for(s = 0;size_t(s) < d->cbs.size() && d->cbs[size_t(s)].used;++s) {}
         if(size_t(s) == d->cbs.size()) d->cbs.emplace_back();
@@ -738,7 +693,7 @@ int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_ca
     // the kernel reads the samples from the update's arena: the record carries the format, and
     // zeros to read should a voice ever meet it without a plan
     h = BufferRec{};
-    h.data = d->d_cb_zero;
+    h.data = d->d_cb_zero.get();
     h.type = adpcm ? uint32_t(B200MIX_FMT_I16) : cb->sample_type;
     h.channels = cb->channels;
     h.pad = uint32_t(s) + 1u;
@@ -766,24 +721,24 @@ int b200mix_buffer_data(b200mix_device *d, uint32_t buffer, uint32_t sample_type
     static const size_t sz[] = {1, 2, 4, 4, 8, 1, 1};
     if(buffer >= d->desc.max_buffers || sample_type > B200MIX_FMT_ALAW || channels < 1 || !data)
     { d->error = "buffer_data: bad arguments"; return B200MIX_ERR_INVALID; }
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     if(int rc = cb_unregister(d, buffer, "buffer_data")) return rc;
     const size_t need = size_t(frames)*channels*sz[sample_type];
     if(bytes < need) { d->error = "buffer_data: short data"; return B200MIX_ERR_INVALID; }
-    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     BufferRec &h = d->h_buffers[buffer];
     if(h.data && d->h_bufrefs[buffer])
     { d->error = "buffer_data: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
+    DevArray<char> &store = d->buf_store[buffer];
     if(h.data)
     {
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        cudaFree(const_cast<void*>(h.data));
+        store.reset();
         h = BufferRec{};
     }
-    void *p = nullptr;
     // +16 bytes so vector/tail reads past the last frame stay inside the allocation
-    CUDA_TRY(d, cudaMalloc(&p, need + 16));
-    CUDA_TRY(d, cudaMemcpyAsync(p, data, need, cudaMemcpyHostToDevice, d->stream));
-    h.data = p; h.frames = frames; h.type = sample_type; h.channels = channels;
+    CUDA_TRY(d, store.alloc(need + 16));
+    CUDA_TRY(d, cudaMemcpyAsync(store.get(), data, need, cudaMemcpyHostToDevice, d->stream));
+    h.data = store.get(); h.frames = frames; h.type = sample_type; h.channels = channels;
     CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec), cudaMemcpyHostToDevice,
         d->stream));
     return B200MIX_OK;
@@ -821,7 +776,7 @@ int b200mix_buffer_free(b200mix_device *d, uint32_t buffer)
     if(h.data)
     {
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        cudaFree(const_cast<void*>(h.data));
+        d->buf_store[buffer].reset();
         h = BufferRec{};
         CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec),
             cudaMemcpyHostToDevice, d->stream));
@@ -852,18 +807,14 @@ static int update_stages(b200mix_device *d)
         d->h_slots[sl].target = d->h_target[sl];
     }
     if(ns && d->d_slots)
-    {
-        CUDA_TRY(d, cudaMemcpyAsync(d->d_slots, d->h_slots.data(), ns*sizeof(SlotRec), cudaMemcpyHostToDevice, d->stream));
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    }
+        if(int rc = upload(d, d->d_slots, d->h_slots)) return rc;
     if(ns && d->d_efx_views)
     {
         std::vector<EfxSlotView> views(ns, EfxSlotView{nullptr, nullptr, 0u, 0u});
         for(uint32_t sl = 0;sl < ns;++sl)
             if(d->h_slots[sl].type >= B200MIX_EFFECT_ECHO && sl < d->efx.size() && d->efx[sl].used)
                 views[sl] = EfxSlotView{d->efx[sl].dev, d->h_slots[sl].lines, d->h_slots[sl].stage, 0u};
-        CUDA_TRY(d, cudaMemcpyAsync(d->d_efx_views, views.data(), ns*sizeof(EfxSlotView), cudaMemcpyHostToDevice, d->stream));
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+        if(int rc = upload(d, d->d_efx_views, views)) return rc;
     }
     return B200MIX_OK;
 }
@@ -871,7 +822,6 @@ static int update_stages(b200mix_device *d)
 static void free_slot(b200mix_device *d, uint32_t slot)
 {
     cudaStreamSynchronize(d->stream);
-    for(void *p : d->slot_allocs[slot]) cudaFree(p);
     d->slot_allocs[slot].clear();
     if(d->h_slots[slot].type) --d->active_slots;
     if(d->h_slots[slot].type == B200MIX_EFFECT_REVERB) --d->reverb_slots;
@@ -881,7 +831,7 @@ static void free_slot(b200mix_device *d, uint32_t slot)
         if(d->h_slots[slot].type == B200MIX_EFFECT_PSHIFTER) --d->pshift_slots;
         if(slot < d->efx.size()) d->efx[slot] = b200mix_device::EfxHost{};
     }
-    if(slot < d->rv.size()) d->rv[slot].used = false;
+    if(slot < d->rv.size()) d->rv[slot] = b200mix_device::RvHost{};
     d->h_slots[slot] = SlotRec{};
     // the device's record goes with it: an install that fails half-way must not leave the old
     // record pointing at freed lines
@@ -913,11 +863,7 @@ int b200mix_slot_convolution(b200mix_device *d, uint32_t slot, uint32_t ir_chann
     // mNumConvolveSegs (alc/effects/convolution.cpp:375-376)
     const uint32_t nseg = std::max<uint32_t>((ir_frames + kConvBlock - 1)/kConvBlock, 2u) - 1u;
     r.segs = nseg;
-    auto alloc = [&](auto *&p, size_t count) -> int {
-        if(int rc = dev_alloc(d, p, count)) return rc;
-        d->slot_allocs[slot].push_back(p);
-        return B200MIX_OK;
-    };
+    auto alloc = [&](auto *&p, size_t count) { return slot_alloc(d, slot, p, count); };
     if(int rc = alloc(r.H, size_t(ir_channels)*nseg*kConvFft)) return rc;
     if(int rc = alloc(r.X, size_t(nseg + kConvMaxBlocks)*kConvFft)) return rc;
     if(int rc = alloc(r.head, size_t(ir_channels)*kConvBlock)) return rc;
@@ -1049,11 +995,7 @@ int b200mix_slot_reverb(b200mix_device *d, uint32_t slot, const b200mix_reverb_p
     R = b200mix_device::RvHost{};
     SlotRec r{};
     r.type = B200MIX_EFFECT_REVERB; r.channels = 16;       // 2 pipeline objects x (4 early + 4 late) lines
-    auto alloc = [&](auto *&ptr, size_t count) -> int {
-        if(int rc = dev_alloc(d, ptr, count)) return rc;
-        d->slot_allocs[slot].push_back(ptr);
-        return B200MIX_OK;
-    };
+    auto alloc = [&](auto *&ptr, size_t count) { return slot_alloc(d, slot, ptr, count); };
     float *main_d = nullptr;
     if(int rc = alloc(main_d, size_t(4)*p->main_len)) return rc;
     for(int obj = 0;obj < 2;++obj)
@@ -1084,8 +1026,8 @@ int b200mix_slot_reverb(b200mix_device *d, uint32_t slot, const b200mix_reverb_p
     }
     reverb_fill_params(R.h[1], p);
     R.fade[1] = p->fade_samples; R.fade[0] = 1u;
-    if(int rc = alloc(R.dev, 2)) return rc;
-    r.H = reinterpret_cast<float*>(R.dev);         // SlotRec::H carries the ReverbDev[2] block
+    CUDA_TRY(d, R.dev.alloc(2, d->stream));
+    r.H = reinterpret_cast<float*>(R.dev.get());   // SlotRec::H carries the ReverbDev[2] block
     if(int rc = alloc(r.lines, size_t(16)*kLine)) return rc;
     if(int rc = alloc(r.gains, size_t(2)*16*32)) return rc;
     if(int rc = alloc(r.gtgt, size_t(16)*32)) return rc;
@@ -1118,7 +1060,7 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
     if(!d->efx_ready) { CUDA_TRY(d, efx_kernels_init()); d->efx_ready = true; }
     if(d->efx.size() < d->h_slots.size()) d->efx.resize(d->h_slots.size());
     if(!d->d_efx_views)
-        if(int rc = dev_alloc(d, d->d_efx_views, d->h_slots.size())) return rc;
+        CUDA_TRY(d, d->d_efx_views.alloc(d->h_slots.size(), d->stream));
     b200mix_device::EfxHost &H = d->efx[slot];
     const bool fresh = !H.used || d->h_slots[slot].type != props->type || H.p.lines != P.lines
         || H.p.echo_len != P.echo_len || H.p.cho_len != P.cho_len;
@@ -1131,13 +1073,9 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
         free_slot(d, slot);
         SlotRec r{};
         r.type = props->type; r.channels = P.lines; r.fade_len = P.fade_len;
-        auto alloc = [&](auto *&ptr, size_t count) -> int {
-            if(int rc = dev_alloc(d, ptr, count)) return rc;
-            d->slot_allocs[slot].push_back(ptr);
-            return B200MIX_OK;
-        };
-        EfxDev *dev = nullptr;
-        if(int rc = alloc(dev, 1)) return rc;
+        auto alloc = [&](auto *&ptr, size_t count) { return slot_alloc(d, slot, ptr, count); };
+        H = b200mix_device::EfxHost{};
+        CUDA_TRY(d, H.dev.alloc(1, d->stream));
         if(int rc = alloc(r.lines, size_t(P.lines)*kLine)) return rc;
         if(int rc = alloc(r.gains, size_t(2)*P.lines*32)) return rc;
         if(int rc = alloc(r.gtgt, size_t(P.lines)*32)) return rc;
@@ -1160,11 +1098,10 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
             if(int rc = alloc(h.ps_sum, size_t(513))) return rc;
             h.ps_count = 0u; h.ps_pos = 1024u - 128u;
         }
-        r.H = reinterpret_cast<float*>(dev);
-        CUDA_TRY(d, cudaMemcpyAsync(dev, &h, sizeof(h), cudaMemcpyHostToDevice, d->stream));
+        r.H = reinterpret_cast<float*>(H.dev.get());
+        CUDA_TRY(d, cudaMemcpyAsync(H.dev, &h, sizeof(h), cudaMemcpyHostToDevice, d->stream));
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        H = b200mix_device::EfxHost{};
-        H.used = true; H.dev = dev; H.mod_index = 0u; H.mod_range = P.mod_range ? P.mod_range : 1u;
+        H.used = true; H.mod_index = 0u; H.mod_range = P.mod_range ? P.mod_range : 1u;
         H.lfo_offset = 0u; H.lfo_range = P.cho_lfo_range ? P.cho_lfo_range : 1u;
         d->h_slots[slot] = r;
         ++d->active_slots; ++d->efx_slots;
@@ -1182,7 +1119,7 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
         {
             H.mod_index = uint32_t(uint64_t(H.mod_index) * P.mod_range_new / H.mod_range);
             H.mod_range = P.mod_range;
-            CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev) + offsetof(EfxDev, mod_index), &H.mod_index,
+            CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev.get()) + offsetof(EfxDev, mod_index), &H.mod_index,
                 sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
         }
         if(props->type == B200MIX_EFFECT_CHORUS)
@@ -1190,7 +1127,7 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
             // mLfoOffset follows the LFO range (chorus.cpp:185-211)
             H.lfo_offset = P.cho_rate_on ? H.lfo_offset * P.cho_lfo_range_new / H.lfo_range : 0u;
             H.lfo_range = P.cho_lfo_range;
-            CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev) + offsetof(EfxDev, cho_lfo_offset), &H.lfo_offset,
+            CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev.get()) + offsetof(EfxDev, cho_lfo_offset), &H.lfo_offset,
                 sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
         }
         if(props->type == B200MIX_EFFECT_FSHIFTER)
@@ -1198,13 +1135,13 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
             static const uint32_t zero = 0u;
             for(int c = 0;c < 4;++c)
                 if(P.fs_reset_phase[c])
-                    CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev) + offsetof(EfxDev, fs_phase) + c*sizeof(uint32_t),
+                    CUDA_TRY(d, cudaMemcpyAsync(reinterpret_cast<char*>(H.dev.get()) + offsetof(EfxDev, fs_phase) + c*sizeof(uint32_t),
                         &zero, sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
         }
         if(props->type == B200MIX_EFFECT_VMORPHER)
             // update() installs newly constructed formant filters: their histories restart at 0
             // (vmorpher.cpp:252-260)
-            CUDA_TRY(d, cudaMemsetAsync(reinterpret_cast<char*>(H.dev) + offsetof(EfxDev, vm_s), 0,
+            CUDA_TRY(d, cudaMemsetAsync(reinterpret_cast<char*>(H.dev.get()) + offsetof(EfxDev, vm_s), 0,
                 sizeof(EfxDev::vm_s), d->stream));
         d->h_slots[slot].fade_len = P.fade_len;
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
@@ -1300,8 +1237,7 @@ int b200mix_hrtf_attach(b200mix_device *d, const b200mix_hrtf *h)
     { d->error = "hrtf_attach: data set HRIRs are longer than the device's ir_size"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    cudaFree(d->d_st_fields); cudaFree(d->d_st_elevs); cudaFree(d->d_st_coeffs); cudaFree(d->d_st_delays);
-    d->d_st_fields = nullptr; d->d_st_elevs = nullptr; d->d_st_coeffs = nullptr; d->d_st_delays = nullptr;
+    d->d_st_fields.reset(); d->d_st_elevs.reset(); d->d_st_coeffs.reset(); d->d_st_delays.reset();
     std::vector<float2> fields(h->fields.size());
     for(size_t i = 0;i < fields.size();++i)
     {
@@ -1311,10 +1247,10 @@ int b200mix_hrtf_attach(b200mix_device *d, const b200mix_hrtf *h)
     }
     std::vector<uint2> elevs(h->elevs.size());
     for(size_t i = 0;i < elevs.size();++i) elevs[i] = make_uint2(h->elevs[i].az_count, h->elevs[i].ir_offset);
-    if(int rc = dev_alloc(d, d->d_st_fields, fields.size(), false)) return rc;
-    if(int rc = dev_alloc(d, d->d_st_elevs, elevs.size(), false)) return rc;
-    if(int rc = dev_alloc(d, d->d_st_coeffs, h->coeffs.size()/2, false)) return rc;
-    if(int rc = dev_alloc(d, d->d_st_delays, h->delays.size(), false)) return rc;
+    CUDA_TRY(d, d->d_st_fields.alloc(fields.size()));
+    CUDA_TRY(d, d->d_st_elevs.alloc(elevs.size()));
+    CUDA_TRY(d, d->d_st_coeffs.alloc(h->coeffs.size()/2));
+    CUDA_TRY(d, d->d_st_delays.alloc(h->delays.size()));
     CUDA_TRY(d, cudaMemcpy(d->d_st_fields, fields.data(), fields.size()*sizeof(float2), cudaMemcpyHostToDevice));
     CUDA_TRY(d, cudaMemcpy(d->d_st_elevs, elevs.data(), elevs.size()*sizeof(uint2), cudaMemcpyHostToDevice));
     CUDA_TRY(d, cudaMemcpy(d->d_st_coeffs, h->coeffs.data(), h->coeffs.size()*sizeof(float), cudaMemcpyHostToDevice));
@@ -1376,12 +1312,10 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     if(!params) { d->error = "voices_update: null params"; return B200MIX_ERR_INVALID; }
     const b200mix_device_desc &dd = d->desc;
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(d->stage_busy)
-    {
-        CUDA_TRY(d, cudaEventSynchronize(d->stage_done));
-        d->stage_busy = false;
-    }
+    CUDA_TRY(d, d->stage.wait());
     if(int rc = ensure_stage(d, n)) return rc;
+    d->stage.begin();
+    VoiceUpdate *const upd = d->stage.host_part<VoiceUpdate>(n);
 
     for(uint32_t i = 0;i < n;++i)
     {
@@ -1414,14 +1348,10 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
                 if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames)
                 { d->error = "voices_update: loop end beyond the buffer"; return B200MIX_ERR_INVALID; }
             }
-            else if(!d->d_qhdr)
-            {
-                // a streaming voice reads its queue: make sure the (empty) queue table exists
-                if(int rc = dev_alloc(d, d->d_qhdr, dd.max_voices)) return rc;
-                if(int rc = dev_alloc(d, d->d_queue, size_t(dd.max_voices)*kMaxQueue)) return rc;
-            }
+            // a streaming voice reads its queue: make sure the (empty) queue table exists
+            else if(int rc = ensure_queues(d)) return rc;
         }
-        VoiceUpdate &u = d->h_upd[i];
+        VoiceUpdate &u = upd[i];
         u.voice = p.voice; u.flags = p.flags; u.buffer = p.buffer; u.resampler = p.resampler;
         if(nobuf) { u.flags |= kUpNoBuffer; u.buffer = 0u; }
         u.position = p.position; u.position_frac = p.position_frac;
@@ -1510,14 +1440,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     if(d->cb_bound)
         if(int rc = cb_group(d)) return rc;
     ApplyParams A{};
-    A.voices = d->d_voices; A.updates = reinterpret_cast<const VoiceUpdate*>(d->d_arena);
-    size_t off = align16(size_t(n)*sizeof(VoiceUpdate));
-    auto pack = [&](const float *src, size_t count) -> const float* {
-        std::memcpy(d->h_arena + off, src, count*sizeof(float));
-        const float *dev = reinterpret_cast<const float*>(d->d_arena + off);
-        off += align16(count*sizeof(float));
-        return dev;
-    };
+    A.voices = d->d_voices; A.updates = d->stage.dev_of(upd);
+    auto pack = [d](const float *src, size_t count) { return d->stage.pack(src, count); };
     if(dirs && dd.ir_size)
     {
         A.dirs = reinterpret_cast<const float4*>(pack(dirs, size_t(n)*4));
@@ -1530,7 +1454,7 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         A.dry = pack(dry_gains, size_t(n)*dd.dry_channels);
     if(send_gains && dd.num_sends && dd.wet_channels)
         A.send = pack(send_gains, size_t(n)*dd.num_sends*dd.wet_channels);
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_arena, d->h_arena, off, cudaMemcpyHostToDevice, d->stream));
+    CUDA_TRY(d, d->stage.ship(d->stream));
     A.hrtf_tgt = d->d_hrtf_tgt; A.hrtf_old = d->d_hrtf_old;
     A.dry_cur = d->d_dry_cur; A.dry_tgt = d->d_dry_tgt;
     A.send_cur = d->d_send_cur; A.send_tgt = d->d_send_tgt;
@@ -1541,8 +1465,6 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     k_apply_updates<<<n, 64, 0, d->stream>>>(A);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
-    CUDA_TRY(d, cudaEventRecord(d->stage_done, d->stream));
-    d->stage_busy = true;
     return B200MIX_OK;
 }
 
@@ -1607,11 +1529,7 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
                 if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames)
                 { d->error = "sources_update: loop end beyond the buffer"; return B200MIX_ERR_INVALID; }
             }
-            else if(!d->d_qhdr)
-            {
-                if(int rc = dev_alloc(d, d->d_qhdr, dd.max_voices)) return rc;
-                if(int rc = dev_alloc(d, d->d_queue, size_t(dd.max_voices)*kMaxQueue)) return rc;
-            }
+            else if(int rc = ensure_queues(d)) return rc;
         }
         for(uint32_t s = 0;s < dd.num_sends;++s)
             if(p.send_slot[s] != B200MIX_NO_SLOT && p.send_slot[s] >= dd.max_slots)
@@ -1668,33 +1586,21 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
 
     // staging: [voices n][props n] in, [VoiceUpdate n][dirs n][dry][send][hf/lf][FilterUpdate] scratch
     const uint32_t paths = 1u + dd.num_sends;
-    const size_t inBytes = align16(size_t(n)*sizeof(b200mix_source_voice)) + align16(size_t(n)*sizeof(b200mix_source_props));
-    if(d->src_busy) { CUDA_TRY(d, cudaEventSynchronize(d->src_done)); d->src_busy = false; }
-    if(n > d->src_cap)
+    CUDA_TRY(d, d->src.wait());
     {
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        if(d->h_src) cudaFreeHost(d->h_src);
-        cudaFree(d->d_src); d->h_src = nullptr; d->d_src = nullptr;
-        const uint32_t cap = std::max(n, 2u*d->src_cap);
+        const uint32_t cap = std::max<uint32_t>(n, 2u*uint32_t(d->src.capacity()));
         const size_t in = align16(size_t(cap)*sizeof(b200mix_source_voice)) + align16(size_t(cap)*sizeof(b200mix_source_props));
         const size_t out = align16(size_t(cap)*sizeof(VoiceUpdate)) + align16(size_t(cap)*16)
             + align16(size_t(cap)*std::max(dd.dry_channels, 1u)*4) + align16(size_t(cap)*std::max(dd.num_sends*dd.wet_channels, 1u)*4)
             + align16(size_t(cap)*(1u + B200MIX_MAX_SENDS)*8) + align16(size_t(cap)*paths*sizeof(FilterUpdate));
-        CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_src), in));
-        CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_src), in + out + 64));
-        if(!d->src_done) CUDA_TRY(d, cudaEventCreateWithFlags(&d->src_done, cudaEventDisableTiming));
-        d->src_cap = cap;
+        CUDA_TRY(d, d->src.reserve(n, cap, in, in + out + 64, d->stream));
     }
-    std::memcpy(d->h_src, voices, size_t(n)*sizeof(b200mix_source_voice));
-    const size_t offProps = align16(size_t(n)*sizeof(b200mix_source_voice));
-    std::memcpy(d->h_src + offProps, props, size_t(n)*sizeof(b200mix_source_props));
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_src, d->h_src, inBytes, cudaMemcpyHostToDevice, d->stream));
-    CUDA_TRY(d, cudaEventRecord(d->src_done, d->stream));
-    d->src_busy = true;
-
+    UploadArena &U = d->src;
+    U.begin();
     CalcVoicesParams Q{};
-    Q.voices = reinterpret_cast<const b200mix_source_voice*>(d->d_src);
-    Q.props = reinterpret_cast<const b200mix_source_props*>(d->d_src + offProps);
+    Q.voices = U.pack(voices, n);
+    Q.props = U.pack(props, n);
+    CUDA_TRY(d, U.ship(d->stream));
     Q.n = n; Q.listener = *listener;
     Q.device_rate = env->device_rate; Q.num_sends = dd.num_sends; Q.render_mode = env->render_mode;
     Q.cd = dd.dry_channels; Q.cw = dd.wet_channels; Q.ir = dd.ir_size;
@@ -1713,15 +1619,12 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
         Q.bsinc[t].scaleBase = d->bsinc[t].scaleBase; Q.bsinc[t].scaleRange = d->bsinc[t].scaleRange;
         for(unsigned k = 0;k < kBsincScales;++k) { Q.bsinc[t].m[k] = d->bsinc[t].m[k]; Q.bsinc[t].filterOffset[k] = d->bsinc[t].filterOffset[k]; }
     }
-    size_t off = inBytes;
-    auto carve = [&](size_t bytes) { char *p = d->d_src + off; off += align16(bytes); return p; };
-    Q.updates = reinterpret_cast<VoiceUpdate*>(carve(size_t(n)*sizeof(VoiceUpdate)));
-    Q.dirs = reinterpret_cast<float4*>(carve(size_t(n)*16));
-    Q.dry = reinterpret_cast<float*>(carve(size_t(n)*std::max(dd.dry_channels, 1u)*4));
-    Q.send = (dd.num_sends && dd.wet_channels)
-        ? reinterpret_cast<float*>(carve(size_t(n)*dd.num_sends*dd.wet_channels*4)) : nullptr;
-    Q.gains_hflf = reinterpret_cast<float*>(carve(size_t(n)*(1u + B200MIX_MAX_SENDS)*8));
-    Q.fupd = reinterpret_cast<FilterUpdate*>(carve(size_t(n)*paths*sizeof(FilterUpdate)));
+    Q.updates = U.carve<VoiceUpdate>(n);
+    Q.dirs = U.carve<float4>(n);
+    Q.dry = U.carve<float>(size_t(n)*std::max(dd.dry_channels, 1u));
+    Q.send = (dd.num_sends && dd.wet_channels) ? U.carve<float>(size_t(n)*dd.num_sends*dd.wet_channels) : nullptr;
+    Q.gains_hflf = U.carve<float>(size_t(n)*(1u + B200MIX_MAX_SENDS)*2);
+    Q.fupd = U.carve<FilterUpdate>(size_t(n)*paths);
     const bool filters = d->d_filt != nullptr;
     CUDA_TRY(d, launch_calc_voices(Q, filters, d->stream));
     d->launches += filters ? 2 : 1;
@@ -1817,11 +1720,7 @@ int b200mix_voice_queue(b200mix_device *d, uint32_t voice, uint32_t count, const
         Q.items[i] = buffers[i];
     }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(!d->d_qhdr)
-    {
-        if(int rc = dev_alloc(d, d->d_qhdr, dd.max_voices)) return rc;
-        if(int rc = dev_alloc(d, d->d_queue, size_t(dd.max_voices)*kMaxQueue)) return rc;
-    }
+    if(int rc = ensure_queues(d)) return rc;
     k_set_queue<<<1, 32, 0, d->stream>>>(d->d_voices, d->d_qhdr, d->d_queue, Q);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
@@ -1836,17 +1735,15 @@ static int ensure_filters(b200mix_device *d)
     const b200mix_device_desc &dd = d->desc;
     const uint32_t paths = 1u + dd.num_sends;
     const size_t count = size_t(dd.max_voices)*paths;
-    if(int rc = dev_alloc(d, d->d_filt, count, false)) return rc;
-    k_filter_init<<<unsigned((count*32u + 255u)/256u), 256, 0, d->stream>>>(d->d_filt, count);
-    ++d->launches;
+    if(int rc = ensure_park_lines(d)) return rc;
+    DevArray<FilterRec> filt; DevArray<float> dline; DevArray<uint32_t> order2;
+    CUDA_TRY(d, filt.alloc(count));
+    CUDA_TRY(d, dline.alloc(size_t(dd.max_voices)*kLine, d->stream));
+    CUDA_TRY(d, order2.alloc(dd.max_voices, d->stream));
+    k_filter_init<<<unsigned((count*32u + 255u)/256u), 256, 0, d->stream>>>(filt, count);
     CUDA_TRY(d, cudaGetLastError());
-    CUDA_TRY(d, cudaEventCreateWithFlags(&d->fstage_done, cudaEventDisableTiming));
-    if(!d->d_xscratch)
-        if(int rc = dev_alloc(d, d->d_xscratch, size_t(dd.max_voices)*kLine)) return rc;
-    if(!d->d_sendinfo)
-        if(int rc = dev_alloc(d, d->d_sendinfo, dd.max_voices)) return rc;
-    if(int rc = dev_alloc(d, d->d_dline, size_t(dd.max_voices)*kLine)) return rc;
-    if(int rc = dev_alloc(d, d->d_order2, dd.max_voices)) return rc;
+    ++d->launches;
+    d->d_filt = std::move(filt); d->d_dline = std::move(dline); d->d_order2 = std::move(order2);
     d->h_dfilt.assign(dd.max_voices, 0);
     return B200MIX_OK;
 }
@@ -1870,30 +1767,16 @@ int b200mix_voices_filters(b200mix_device *d, uint32_t n, const b200mix_voice_fi
             const uint8_t act = filters[i].active ? 1 : 0;
             if(d->h_dfilt[filters[i].voice] != act) { d->h_dfilt[filters[i].voice] = act; d->order2_dirty = true; }
         }
-    if(d->fstage_busy)
-    {
-        CUDA_TRY(d, cudaEventSynchronize(d->fstage_done));
-        d->fstage_busy = false;
-    }
-    if(n > d->fupd_cap)
-    {
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        if(d->h_fupd) cudaFreeHost(d->h_fupd);
-        cudaFree(d->d_fupd);
-        d->h_fupd = nullptr; d->d_fupd = nullptr;
-        const uint32_t cap = std::max(n, 2u*d->fupd_cap);
-        CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_fupd), size_t(cap)*sizeof(FilterUpdate)));
-        CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_fupd), size_t(cap)*sizeof(FilterUpdate)));
-        d->fupd_cap = cap;
-    }
-    std::memcpy(d->h_fupd, filters, size_t(n)*sizeof(FilterUpdate));
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_fupd, d->h_fupd, size_t(n)*sizeof(FilterUpdate),
-        cudaMemcpyHostToDevice, d->stream));
-    k_apply_filter_updates<<<(2u*n + 127u)/128u, 128, 0, d->stream>>>(d->d_filt, paths, d->d_fupd, n);
+    UploadArena &U = d->fstage;
+    CUDA_TRY(d, U.wait());
+    const size_t cap = std::max<size_t>(n, 2u*U.capacity());
+    CUDA_TRY(d, U.reserve(n, cap, cap*sizeof(FilterUpdate), cap*sizeof(FilterUpdate), d->stream));
+    U.begin();
+    const FilterUpdate *fupd = U.pack(reinterpret_cast<const FilterUpdate*>(filters), n);
+    CUDA_TRY(d, U.ship(d->stream));
+    k_apply_filter_updates<<<(2u*n + 127u)/128u, 128, 0, d->stream>>>(d->d_filt, paths, fupd, n);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
-    CUDA_TRY(d, cudaEventRecord(d->fstage_done, d->stream));
-    d->fstage_busy = true;
     return B200MIX_OK;
 }
 
@@ -1984,27 +1867,14 @@ static int cb_plan_update(b200mix_device *d, uint32_t frames, const BufferRec *&
         w.region = size + pad;
         size = w.region + align16(w.bytes) + pad;
     }
-    // 2. the arenas (the pinned one alternates: the other may still be in flight)
-    const int k = d->cb_idx;
-    if(d->cb_busy[k]) { CUDA_TRY(d, cudaEventSynchronize(d->cb_done[k])); d->cb_busy[k] = false; }
-    if(!d->cb_done[k]) CUDA_TRY(d, cudaEventCreateWithFlags(&d->cb_done[k], cudaEventDisableTiming));
-    if(size > d->h_cb_cap[k])
-    {
-        if(d->h_cb[k]) cudaFreeHost(d->h_cb[k]);
-        d->h_cb[k] = nullptr; d->h_cb_cap[k] = 0;
-        CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&d->h_cb[k]), size*2));
-        d->h_cb_cap[k] = size*2;
-    }
-    if(size > d->d_cb_cap)
-    {
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));     // the last update may still read it
-        cudaFree(d->d_cb);
-        d->d_cb = nullptr; d->d_cb_cap = 0;
-        CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_cb), size*2));
-        d->d_cb_cap = size*2;
-    }
+    // 2. the arena (two alternate: the other one's copy may still be in flight)
+    UploadArena &U = d->cb_arena[d->cb_idx];
+    CUDA_TRY(d, U.wait());
+    CUDA_TRY(d, U.reserve(size, size*2, size*2, size*2, d->stream));
+    U.begin();
+    uint8_t *arena = U.host_part<uint8_t>(size);
+    const uintptr_t devArena = reinterpret_cast<uintptr_t>(U.dev_of(arena));
     // 3. pack, then what the reference does after the mix
-    uint8_t *arena = reinterpret_cast<uint8_t*>(d->h_cb[k]);
     std::memset(arena, 0, size);
     for(size_t s = 0;s < d->cbs.size();++s)
     {
@@ -2015,7 +1885,7 @@ static int cb_plan_update(b200mix_device *d, uint32_t frames, const BufferRec *&
         cbplan::Voice &vm = d->cbv[size_t(reps[s])].v;
         const cbplan::Span span = cbplan::span_of(w.start, vm, cb.samples_per_block, c.st);
         BufferRec rec = d->h_buffers[c.buffer];
-        rec.data = reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(d->d_cb)
+        rec.data = reinterpret_cast<const void*>(devArena
             + uintptr_t(int64_t(w.region) + span.base*int64_t(c.frame_bytes)));
         rec.frames = w.loads.chunks ? span.frames : 0u;
         std::memcpy(arena + s*sizeof(BufferRec), &rec, sizeof(rec));
@@ -2035,11 +1905,9 @@ static int cb_plan_update(b200mix_device *d, uint32_t frames, const BufferRec *&
         // the source's other channel voices move with it
         for(uint32_t v : d->cb_members[s]) d->cbv[v].v = vm;
     }
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_cb, arena, size, cudaMemcpyHostToDevice, d->stream));
-    CUDA_TRY(d, cudaEventRecord(d->cb_done[k], d->stream));
-    d->cb_busy[k] = true;
-    d->cb_idx = k ^ 1;
-    plan = reinterpret_cast<const BufferRec*>(d->d_cb);
+    CUDA_TRY(d, U.ship(d->stream));
+    d->cb_idx ^= 1;
+    plan = reinterpret_cast<const BufferRec*>(devArena);
     return B200MIX_OK;
 }
 
@@ -2081,12 +1949,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             [d](uint32_t a, uint32_t b) { return d->h_cost[a] > d->h_cost[b]; });
         d->num_order = uint32_t(d->h_order.size());
         if(d->num_order)
-        {
-            // the vector may be reused before the copy completes: synchronise (rare path)
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_order, d->h_order.data(), d->num_order*sizeof(uint32_t),
-                cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        }
+            if(int rc = upload(d, d->d_order, d->h_order)) return rc;
         d->order_dirty = false;
         d->order2_dirty = true;
         d->dry_entries_dirty = true;
@@ -2099,11 +1962,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         for(uint32_t v : d->h_order) if(d->dev_filters || d->h_dfilt[v]) d->h_order2.push_back(v);
         d->num_order2 = uint32_t(d->h_order2.size());
         if(d->num_order2)
-        {
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_order2, d->h_order2.data(), d->num_order2*sizeof(uint32_t),
-                cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        }
+            if(int rc = upload(d, d->d_order2, d->h_order2)) return rc;
         d->order2_dirty = false;
     }
     const bool hrtfDev = dd.ir_size > 0;
@@ -2209,10 +2068,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             d->num_dry_entries = uint32_t(d->h_dry_entries.size());
             const uint32_t ss[2] = {0u, d->num_dry_entries};
             CUDA_TRY(d, cudaMemcpyAsync(d->d_dry_slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, d->stream));
-            if(d->num_dry_entries)
-                CUDA_TRY(d, cudaMemcpyAsync(d->d_dry_entries, d->h_dry_entries.data(),
-                    d->num_dry_entries*sizeof(SendEntry), cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            if(int rc = upload(d, d->d_dry_entries, d->h_dry_entries)) return rc;
             d->dry_entries_dirty = false;
         }
         if(d->num_dry_entries)
@@ -2259,10 +2115,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
                 d->max_slot_entries = std::max(d->max_slot_entries, d->h_slot_start[sl+1] - d->h_slot_start[sl]);
             CUDA_TRY(d, cudaMemcpyAsync(d->d_slot_start, d->h_slot_start.data(),
                 (dd.max_slots + 1)*sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
-            if(d->num_entries)
-                CUDA_TRY(d, cudaMemcpyAsync(d->d_entries, d->h_entries.data(),
-                    d->num_entries*sizeof(SendEntry), cudaMemcpyHostToDevice, d->stream));
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            if(int rc = upload(d, d->d_entries, d->h_entries)) return rc;
             d->sends_dirty = false;
         }
         SendMixParams SM{};
@@ -2272,14 +2125,10 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         SM.valid_bit = kSiSend;
         if(d->d_filt && d->num_entries)
         {
-            if(d->fscratch_rows < d->num_entries)
+            if(d->d_fscratch.size() < size_t(d->num_entries)*kLine)
             {
-                CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-                cudaFree(d->d_fscratch); d->d_fscratch = nullptr; d->fscratch_rows = 0;
-                const uint32_t rows = std::max(d->num_entries, 64u);
-                CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_fscratch), size_t(rows)*kLine*sizeof(float)));
-                CUDA_TRY(d, cudaMemsetAsync(d->d_fscratch, 0, size_t(rows)*kLine*sizeof(float), d->stream));
-                d->fscratch_rows = rows;
+                CUDA_TRY(d, regrow(d->d_fscratch, size_t(std::max(d->num_entries, 64u))*kLine, d->stream));
+                CUDA_TRY(d, cudaMemsetAsync(d->d_fscratch, 0, d->d_fscratch.bytes(), d->stream));
             }
             SM.filt = d->d_filt; SM.filt_paths = 1u + dd.num_sends; SM.fscratch = d->d_fscratch;
             FilterRunParams FP{};
@@ -2292,14 +2141,9 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         SM.geff = d->d_send_geff; SM.gramp = d->d_send_gramp;
         // a CTA's 8 warps share its entries evenly: chunks of 128 entries per slot
         const uint32_t chunks = std::max(1u, std::min(16u, (d->max_slot_entries + 127u)/128u));
-        if(chunks > 1u && d->send_partial_chunks < chunks)
-        {
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-            cudaFree(d->d_send_partial); d->d_send_partial = nullptr; d->send_partial_chunks = 0;
-            CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&d->d_send_partial),
-                size_t(chunks)*dd.max_slots*dd.wet_channels*kLine*sizeof(float)));
-            d->send_partial_chunks = chunks;
-        }
+        const size_t partialFloats = size_t(chunks)*dd.max_slots*dd.wet_channels*kLine;
+        if(chunks > 1u && d->d_send_partial.size() < partialFloats)
+            CUDA_TRY(d, regrow(d->d_send_partial, partialFloats, d->stream));
         SM.chunks = chunks; SM.partial = d->d_send_partial;
         if(int rc = run_bus_mix(d, SM, d->num_entries, dd.max_slots, false)) return rc;
     }
@@ -2557,7 +2401,7 @@ static int shard_wet_exchange(b200mix_device *d)
         ShardPushParams P{};
         P.src = d->d_wet; P.rank = S.rank; P.world = S.world; P.epoch = S.epoch;
         P.wet = 1u; P.num_slots = dd.max_slots; P.slot_floats = slotFloats; P.owned_max = S.owned_max;
-        P.own = reinterpret_cast<ShardCtl*>(S.own);
+        P.own = reinterpret_cast<ShardCtl*>(S.own.get());
         for(uint32_t r = 0;r < S.world;++r) P.peer[r] = S.peer[r];
         P.off_data = S.off_wet; P.per_src_floats = S.wet_src_floats;
         P.counters = S.d_counters + 4;
@@ -2593,7 +2437,7 @@ static int shard_real_reduce(b200mix_device *d)
     {
         ShardPushParams P{};
         P.src = d->d_real; P.rank = S.rank; P.world = S.world; P.epoch = S.epoch; P.floats = floats;
-        P.own = reinterpret_cast<ShardCtl*>(S.own);
+        P.own = reinterpret_cast<ShardCtl*>(S.own.get());
         for(uint32_t r = 0;r < S.world;++r) P.peer[r] = S.peer[r];
         P.off_data = S.off_real; P.per_src_floats = S.real_floats; P.counters = S.d_counters;
         k_shard_push<<<dim3(std::max(1u, floats/(4u*256u*2u)), 1), 256, 0, d->stream>>>(P);
@@ -2603,7 +2447,7 @@ static int shard_real_reduce(b200mix_device *d)
     {
         ShardSumParams Q{};
         Q.dst = d->d_real; Q.rank = 0u; Q.world = S.world; Q.epoch = S.epoch; Q.floats = floats;
-        Q.own = reinterpret_cast<ShardCtl*>(S.own);
+        Q.own = reinterpret_cast<ShardCtl*>(S.own.get());
         for(uint32_t r = 0;r < S.world;++r) Q.peer[r] = S.peer[r];
         Q.off_data = S.off_real; Q.per_src_floats = S.real_floats; Q.counter = S.d_counters + 1;
         k_shard_sum<<<std::max(1u, floats/(4u*256u*2u)), 256, 0, d->stream>>>(Q);
@@ -2632,7 +2476,7 @@ static int render_collect(b200mix_device *d, uint32_t frames, float *const *real
 {
     const b200mix_device_desc &dd = d->desc;
     const uint32_t nv = std::max(d->voice_hi, 1u);
-    const bool contiguous = d->d_real == reinterpret_cast<float*>(d->d_outblock);
+    const bool contiguous = d->d_real == reinterpret_cast<float*>(d->d_outblock.get());
     if(real_out && results && contiguous)
         CUDA_TRY(d, cudaMemcpyAsync(d->h_outblock, d->d_outblock, d->out_real_bytes + size_t(nv)*sizeof(VoiceResult),
             cudaMemcpyDeviceToHost, d->stream));
@@ -2649,7 +2493,6 @@ static int render_collect(b200mix_device *d, uint32_t frames, float *const *real
         CUDA_TRY(d, cudaMemcpyAsync(d->shard.h_status, d->shard.own + offsetof(ShardCtl, status),
             sizeof(uint32_t), cudaMemcpyDeviceToHost, d->stream));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    d->stage_busy = false;
     if(d->shard.transport == 1 && *d->shard.h_status)
     { d->error = "render: a peer of the sharded device set did not answer in time"; return B200MIX_ERR_CUDA; }
     if(real_out)
@@ -2680,15 +2523,17 @@ int b200mix_set_uhj_encoder(b200mix_device *d, uint32_t filter_length, uint32_t 
         || dd.dry_channels < 3
         || (filter_length != 0 && filter_length != 256 && filter_length != 512))
     { d->error = "set_uhj_encoder: needs a UHJ device and a length of 0, 256 or 512"; return B200MIX_ERR_INVALID; }
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     CUDA_TRY(d, cudaMemset(d->d_uhj_state, 0, 64*sizeof(float)));
     if(filter_length)
     {
         if(!d->d_uhj_fir_state)
         {
-            if(int rc = dev_alloc(d, d->d_uhj_fir_state, kUhjFirStateFloats)) return rc;
-            if(int rc = dev_alloc(d, d->d_uhj_fir_coef, 256)) return rc;
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
+            DevArray<float> state, coef;
+            CUDA_TRY(d, state.alloc(kUhjFirStateFloats));
+            CUDA_TRY(d, coef.alloc(256));
+            d->d_uhj_fir_state = std::move(state); d->d_uhj_fir_coef = std::move(coef);
         }
         CUDA_TRY(d, cudaMemset(d->d_uhj_fir_state, 0, kUhjFirStateFloats*sizeof(float)));
         // SegmentedFilter's desired response (core/allpass_conv.hpp:56-75): Blackman-Nuttall
@@ -2716,6 +2561,7 @@ int b200mix_set_front_stabilizer(b200mix_device *d, uint32_t center_channel, flo
     if(!d) return B200MIX_ERR_INVALID;
     const b200mix_device_desc &dd = d->desc;
     if(d->mid_render) { d->error = "set_front_stabilizer: a render_begin is pending"; return B200MIX_ERR_INVALID; }
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     if(center_channel == B200MIX_NO_SLOT) { d->stab_center = B200MIX_NO_SLOT; return B200MIX_OK; }
     if(dd.post_process != B200MIX_POST_AMBIDEC || center_channel >= dd.real_channels
@@ -2723,10 +2569,7 @@ int b200mix_set_front_stabilizer(b200mix_device *d, uint32_t center_channel, flo
         || center_channel == dd.real_left || center_channel == dd.real_right || dd.real_channels > 32u)
     { d->error = "set_front_stabilizer: needs an ambisonic-decode device with left, right and centre outputs"; return B200MIX_ERR_INVALID; }
     if(!d->d_stab_state)
-    {
-        if(int rc = dev_alloc(d, d->d_stab_state, 4 + 32)) return rc;
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    }
+        CUDA_TRY(d, d->d_stab_state.alloc(4 + 32));
     CUDA_TRY(d, cudaMemset(d->d_stab_state, 0, (4 + 32)*sizeof(float)));
     CUDA_TRY(d, cudaFuncSetAttribute(k_post_stabilizer, cudaFuncAttributeMaxDynamicSharedMemorySize,
         int(size_t(2u + dd.real_channels)*kLine*sizeof(float))));
@@ -2741,10 +2584,11 @@ int b200mix_set_bs2b(b200mix_device *d, uint32_t level)
     if(d->mid_render || level > 6 || dd.post_process != B200MIX_POST_AMBIDEC || dd.real_left == dd.real_right
         || dd.real_left >= dd.real_channels || dd.real_right >= dd.real_channels)
     { d->error = "set_bs2b: needs a stereo ambisonic-decode device and a level of 0..6"; return B200MIX_ERR_INVALID; }
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     if(!d->d_bs2b)
     {
-        if(int rc = dev_alloc(d, d->d_bs2b, 16)) return rc;
+        CUDA_TRY(d, d->d_bs2b.alloc(16, d->stream));
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     }
     float h[9] = {};
@@ -2777,9 +2621,9 @@ int b200mix_set_distance_comp(b200mix_device *d, uint32_t channels, const uint32
     if(!d) return B200MIX_ERR_INVALID;
     if(d->mid_render) { d->error = "set_distance_comp: a render_begin is pending"; return B200MIX_ERR_INVALID; }
     const b200mix_device_desc &dd = d->desc;
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    cudaFree(d->d_dc_delay); cudaFree(d->d_dc_gain); cudaFree(d->d_dc_buf);
-    d->d_dc_delay = nullptr; d->d_dc_gain = nullptr; d->d_dc_buf = nullptr;
+    d->d_dc_delay.reset(); d->d_dc_gain.reset(); d->d_dc_buf.reset();
     if(!channels) return B200MIX_OK;
     if(channels > dd.real_channels || !delays || !gains)
     { d->error = "set_distance_comp: bad arguments"; return B200MIX_ERR_INVALID; }
@@ -2790,12 +2634,15 @@ int b200mix_set_distance_comp(b200mix_device *d, uint32_t channels, const uint32
         if(delays[c] >= kLine) { d->error = "set_distance_comp: delay >= 1024"; return B200MIX_ERR_INVALID; }
         hd[c] = delays[c]; hg[c] = gains[c];
     }
-    if(int rc = dev_alloc(d, d->d_dc_delay, dd.real_channels)) return rc;
-    if(int rc = dev_alloc(d, d->d_dc_gain, dd.real_channels)) return rc;
-    if(int rc = dev_alloc(d, d->d_dc_buf, size_t(dd.real_channels)*kLine)) return rc;
+    // committed only whole: render_output_stage runs the delays when d_dc_delay is set
+    DevArray<uint32_t> delay; DevArray<float> gain, buf;
+    CUDA_TRY(d, delay.alloc(dd.real_channels));
+    CUDA_TRY(d, gain.alloc(dd.real_channels));
+    CUDA_TRY(d, buf.alloc(size_t(dd.real_channels)*kLine, d->stream));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    CUDA_TRY(d, cudaMemcpy(d->d_dc_delay, hd.data(), hd.size()*sizeof(uint32_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(d, cudaMemcpy(d->d_dc_gain, hg.data(), hg.size()*sizeof(float), cudaMemcpyHostToDevice));
+    CUDA_TRY(d, cudaMemcpy(delay, hd.data(), hd.size()*sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CUDA_TRY(d, cudaMemcpy(gain, hg.data(), hg.size()*sizeof(float), cudaMemcpyHostToDevice));
+    d->d_dc_delay = std::move(delay); d->d_dc_gain = std::move(gain); d->d_dc_buf = std::move(buf);
     return B200MIX_OK;
 }
 
@@ -2807,11 +2654,11 @@ int b200mix_set_limiter(b200mix_device *d, const b200mix_limiter_desc *p, uint32
     if(look_ahead) *look_ahead = 0;
     if(d->mid_render) { d->error = "set_limiter: a render_begin is pending"; return B200MIX_ERR_INVALID; }
     const b200mix_device_desc &dd = d->desc;
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     if(!p)
     {
         CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        cudaFree(d->d_limiter); d->d_limiter = nullptr;
-        cudaFree(d->d_limiter_delay); d->d_limiter_delay = nullptr;
+        d->d_limiter.reset(); d->d_limiter_delay.reset();
         return B200MIX_OK;
     }
     if(p->struct_size != sizeof(*p)) { d->error = "set_limiter: struct_size"; return B200MIX_ERR_INVALID; }
@@ -2839,8 +2686,10 @@ int b200mix_set_limiter(b200mix_device *d, const b200mix_limiter_desc *p, uint32
     for(float &v : h.hold_hist) v = -INFINITY;
     if(!d->d_limiter)
     {
-        if(int rc = dev_alloc(d, d->d_limiter, 1)) return rc;
-        if(int rc = dev_alloc(d, d->d_limiter_delay, size_t(std::max(dd.real_channels, 1u))*kLine)) return rc;
+        DevArray<LimiterDev> lim; DevArray<float> delay;
+        CUDA_TRY(d, lim.alloc(1));
+        CUDA_TRY(d, delay.alloc(size_t(std::max(dd.real_channels, 1u))*kLine));
+        d->d_limiter = std::move(lim); d->d_limiter_delay = std::move(delay);
     }
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     CUDA_TRY(d, cudaMemcpy(d->d_limiter, &h, sizeof(h), cudaMemcpyHostToDevice));
@@ -2871,10 +2720,10 @@ int b200mix_render_interleaved(b200mix_device *d, uint32_t frames, void *out, ui
     { d->error = "render_interleaved: bad arguments"; return B200MIX_ERR_INVALID; }
     if(int rc = render_launch(d, frames, results != nullptr)) return rc;
     static const size_t sz[] = {1, 1, 2, 2, 4, 4, 4};
-    if(!d->d_outbuf)
+    if(!d->h_outbuf)
     {
-        CUDA_TRY(d, cudaMalloc(&d->d_outbuf, size_t(kLine)*64*4));
-        CUDA_TRY(d, cudaMallocHost(&d->h_outbuf, size_t(kLine)*64*4));
+        CUDA_TRY(d, d->d_outbuf.alloc(size_t(kLine)*64*4));
+        CUDA_TRY(d, d->h_outbuf.alloc(size_t(kLine)*64*4));
     }
     OutputParams Q{};
     Q.real = d->d_real; Q.out = d->d_outbuf; Q.frames = frames; Q.channels = dd.real_channels;
@@ -2935,9 +2784,6 @@ static void shard_release(b200mix_device *d)
             if(r != S.rank && S.peer[r]) cudaIpcCloseMemHandle(S.peer[r]);
     if(S.comm && S.comm_destroy) S.comm_destroy(S.comm);
     if(S.nccl_lib) dlclose(S.nccl_lib);
-    cudaFree(S.own); cudaFree(S.d_counters);
-    if(S.h_status) cudaFreeHost(S.h_status);
-    for(cudaEvent_t e : S.ev) if(e) cudaEventDestroy(e);
     S = b200mix_device::Shard{};
 }
 
@@ -2950,7 +2796,7 @@ static int shard_common(b200mix_device *d, uint32_t rank, uint32_t world)
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     shard_release(d);
     d->shard.rank = rank; d->shard.world = world;
-    for(cudaEvent_t &e : d->shard.ev) CUDA_TRY(d, cudaEventCreate(&e));
+    for(Event &e : d->shard.ev) CUDA_TRY(d, e.create());
     return B200MIX_OK;
 }
 
@@ -2967,11 +2813,10 @@ int b200mix_shard_init(b200mix_device *d, uint32_t rank, uint32_t world, void *h
     S.wet_src_floats = size_t(S.owned_max)*dd.wet_channels*kLine;
     S.off_real = sizeof(ShardCtl);
     S.off_wet = S.off_real + size_t(2)*world*S.real_floats*sizeof(float);
-    S.bytes = S.off_wet + size_t(2)*world*S.wet_src_floats*sizeof(float);
-    CUDA_TRY(d, cudaMalloc(reinterpret_cast<void**>(&S.own), S.bytes));
-    CUDA_TRY(d, cudaMemset(S.own, 0, S.bytes));
-    if(int rc = dev_alloc(d, S.d_counters, 4 + kShardMaxWorld)) return rc;
-    CUDA_TRY(d, cudaMallocHost(reinterpret_cast<void**>(&S.h_status), sizeof(uint32_t)));
+    CUDA_TRY(d, S.own.alloc(S.off_wet + size_t(2)*world*S.wet_src_floats*sizeof(float)));
+    CUDA_TRY(d, cudaMemset(S.own, 0, S.own.bytes()));
+    CUDA_TRY(d, S.d_counters.alloc(4 + kShardMaxWorld, d->stream));
+    CUDA_TRY(d, S.h_status.alloc(1));
     *S.h_status = 0u;
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     cudaIpcMemHandle_t h;
@@ -2989,7 +2834,7 @@ int b200mix_shard_connect(b200mix_device *d, const void *handles)
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     for(uint32_t r = 0;r < S.world;++r)
     {
-        if(r == S.rank) { S.peer[r] = S.own; continue; }
+        if(r == S.rank) { S.peer[r] = S.own.get(); continue; }
         cudaIpcMemHandle_t h;
         std::memcpy(&h, static_cast<const char*>(handles) + size_t(r)*sizeof(h), sizeof(h));
         void *p = nullptr;
@@ -3117,13 +2962,13 @@ int b200mix_profile(b200mix_device *d, int enable)
 {
     if(!d) return B200MIX_ERR_INVALID;
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(enable && !d->ev_mix0)
+    if(enable && !d->ev_mix1)
     {
-        CUDA_TRY(d, cudaEventCreate(&d->ev_mix0));
-        CUDA_TRY(d, cudaEventCreate(&d->ev_mix1));
+        CUDA_TRY(d, d->ev_mix0.create());
+        CUDA_TRY(d, d->ev_mix1.create());
     }
-    if(enable >= 2 && !d->ev_stage[0])
-        for(cudaEvent_t &e : d->ev_stage) CUDA_TRY(d, cudaEventCreate(&e));
+    if(enable >= 2 && !d->ev_stage[b200mix_device::kStages])
+        for(Event &e : d->ev_stage) CUDA_TRY(d, e.create());
     d->profile = enable != 0;
     d->profile_level = enable;
     d->ev_valid = false; d->stage_valid = false;
