@@ -161,7 +161,8 @@ inline After finish_update(State &s, uint32_t spb, uint32_t bpb, Voice &v, uint3
     const uint32_t samplesDone = frac >> 16;
     v.pos = add_sat(v.pos, int32_t(samplesDone));
     v.frac = frac & 0xffffu;
-    if(!v.have_buffer || v.pos <= 0) return a;
+    if(!v.have_buffer) { v.state = 2u; return a; }     // no buffer: Stopping (voice.cpp:1224-1232)
+    if(v.pos <= 0) return a;
     const uint32_t done = samplesDone < uint32_t(v.pos) ? samplesDone : uint32_t(v.pos);
     const uint32_t endOffset = s.block_offset + done;
     const uint32_t blocksDone = endOffset / spb;

@@ -1026,6 +1026,9 @@ __device__ __forceinline__ void write_back_voice(const MixParams &P, VoiceRec &r
                 newState = 2u;
             }
         }
+        // a voice that had no buffer to begin with stops as well: one that ran out earlier and
+        // was set playing again by an update fades out on the next one (core/voice.cpp:1224-1232)
+        if(!haveBuffer) newState = 2u;
         rec.pos = pos; rec.frac = frac;
     }
     rec.flags = newFlags;

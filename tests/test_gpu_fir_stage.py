@@ -11,10 +11,13 @@ steady ramp.  These scenes reach what that must get right:
     ones;
   - fades with new HRIRs (the old HRIR is staged too), with new delays only (the old-filter pass
     runs on the target HRIR) and with new gains only (one merged pass);
+  - voices that stop (VF_STOPPING) with no new parameters, with new HRIRs (some of them through
+    a direct filter), with new delays and with new gains, and the update after, which mixes
+    only their carried tails;
   - 40 voices, fewer than the kernel has voice groups (one voice per group, none to look ahead
     to), and 3000, which gives groups two or three order slots on a 132-SM H100;
   - HRIR lengths 8, 40, 64, 72 and 128 (both FIR variants).
-Stopping voices stay out: at HRIR lengths other than 64 they have an open parity bug."""
+tests/test_hrtf_stop.py holds stopping voices to a float64 restatement as well."""
 import numpy as np
 import pytest
 
@@ -50,6 +53,9 @@ def _render(lib, nv, ir, seed):
     new_delay = [k for k in live if k % 5 == 2]
     new_gain = [k for k in live if k % 5 == 3]
     filtered = [k for k in live if k % 3 == 0]
+    stop_plain = [k for k in live if k % 10 == 4]          # stopped with no new parameters
+    stop_hrir = [k for k in live if k % 10 == 9]           # stopped with new HRIRs
+    stopping = set(k for k in live if k % 20 in (2, 3))    # stopped with the last new delay / gain
     lp = np.zeros(5, dtype=np.float32)
     hp = np.zeros(5, dtype=np.float32)
     prod = mixlib.product()
@@ -64,15 +70,20 @@ def _render(lib, nv, ir, seed):
         dev.buffer_data(b, abi.FMT_I16, scene.voice_buffer_fast(b, FRAMES))
     dev.voices_update(params, coeffs, dry, None)
 
-    def moved(idx, change):
+    def moved(idx, change, stop=()):
         out = []
         for k in idx:
             q = _copy(params[k])
             q.flags &= ~abi.VF_RESET
+            if k in stop:                                 # fades out over this update
+                q.flags = (q.flags & ~abi.VF_PLAYING) | abi.VF_STOPPING
             change(q)
             params[k] = q
             out.append(q)
         return out
+
+    def same(q):
+        pass
 
     def delay(q):
         q.hrtf_delay[1] = (q.hrtf_delay[1] + 7) % 64
@@ -90,18 +101,25 @@ def _render(lib, nv, ir, seed):
             # new HRIRs, delays and gains: 64-sample fades with the old HRIR
             coeffs[new_hrir] = coeffs[new_hrir][:, ::-1, :] * 0.5
             dev.voices_update(moved(new_hrir, hrir), coeffs[new_hrir], dry[new_hrir], None)
+            # stopping voices: a 64-sample (or n-sample) fade of the old HRIR to silence
+            dev.voices_update(moved(stop_plain, same, stop_plain), None, dry[stop_plain], None)
         if u == 2:
             # same HRIRs: new delays (old-filter pass on the target HRIR), new gains (merged pass)
             dev.voices_update(moved(new_delay, delay), None, dry[new_delay], None)
             dev.voices_update(moved(new_gain, gain), None, dry[new_gain], None)
         if u == 3:
-            # direct filters: these lines come from the filtered lines; some fade as well
+            # direct filters: these lines come from the filtered lines; some fade as well, some
+            # stop with new HRIRs (the old HRIR is staged and faded out)
             dev.voices_filters((k, 0, 1, lp, hp) for k in filtered)
             coeffs[new_hrir] = coeffs[new_hrir] * 0.8
             dev.voices_update(moved(new_hrir, hrir), coeffs[new_hrir], dry[new_hrir], None)
+            coeffs[stop_hrir] = coeffs[stop_hrir][:, ::-1, :] * 0.9
+            dev.voices_update(moved(stop_hrir, hrir, stop_hrir), coeffs[stop_hrir], dry[stop_hrir], None)
         if u == 4:
-            dev.voices_update(moved(new_delay, delay), None, dry[new_delay], None)
-            dev.voices_update(moved(new_gain, gain), None, dry[new_gain], None)
+            # some stop with their new delays or gains; the last update mixes the stopped voices'
+            # carried tails only
+            dev.voices_update(moved(new_delay, delay, stopping), None, dry[new_delay], None)
+            dev.voices_update(moved(new_gain, gain, stopping), None, dry[new_gain], None)
         outs.append(dev.render(frames))
     dev.close()
     return outs

@@ -5,7 +5,8 @@ copy staged.  These scenes reach the cases that path must get right: spans at ev
 (0..7) with even and odd window origins, negative start positions (leading zeros), one-run and
 wrapping loop spans, a buffer that ends inside the window, pitches that need two chunks,
 bsinc12/24/48 and fast bsinc.  The lines go through the HRIR FIR at sizes from 8 to 128 (both FIR
-variants), with coefficient changes mid-run (the old-filter pass) and gain fades."""
+variants), with coefficient changes mid-run (the old-filter pass), gain fades and voices that stop
+(VF_STOPPING) with and without new HRIRs, and the update after the stops."""
 import numpy as np
 import pytest
 
@@ -51,6 +52,7 @@ def _render(lib, ir, seed):
     rng = np.random.default_rng(seed)
     params, coeffs, dry = _voices(rng, ir)
     moved = list(range(0, NV, 3))
+    stopped = list(range(1, NV, 3))
     new_coeffs = coeffs.copy()
     new_coeffs[moved] = coeffs[moved][:, ::-1, :] * 0.5
     dev = MixDevice(lib, synth.hrtf_desc(NV, ir))
@@ -59,17 +61,28 @@ def _render(lib, ir, seed):
         dev.buffer_data(i, abi.FMT_I16, scene.voice_buffer_fast(i, FRAMES))
     dev.voices_update(params, coeffs, dry, None)
     outs = []
-    for u in range(2):
+    for u in range(3):
         if u == 1:
-            # new HRIRs, delays and gains without a reset: 64-sample fades, old-filter pass
+            # new HRIRs, delays and gains without a reset: 64-sample fades, old-filter pass;
+            # every other one of these stops as well (its old HRIR fades out)
             upd = []
             for k in moved:
                 p = params[k]
                 p.flags &= ~abi.VF_RESET
+                if k % 2:
+                    p.flags = (p.flags & ~abi.VF_PLAYING) | abi.VF_STOPPING
                 p.hrtf_delay[0] = (p.hrtf_delay[0] + 5) % 64
                 p.hrtf_gain *= 0.7
                 upd.append(p)
             dev.voices_update(upd, new_coeffs[moved], dry[moved], None)
+            # stopped with no new parameters
+            upd = []
+            for k in stopped:
+                p = params[k]
+                p.flags = (p.flags & ~(abi.VF_RESET | abi.VF_PLAYING)) | abi.VF_STOPPING
+                upd.append(p)
+            dev.voices_update(upd, None, dry[stopped], None)
+        # u == 2: the stopped voices leave only their carried tails
         outs.append(dev.render(1024))
     dev.close()
     return outs
