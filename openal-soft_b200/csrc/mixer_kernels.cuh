@@ -124,6 +124,26 @@ __device__ __forceinline__ void group_sync(int id, int count)
     else asm volatile("bar.sync 2, %0;" :: "r"(count) : "memory");
 }
 
+// group_sync that also returns whether pred holds on every thread of the group (bar.red.and)
+__device__ __forceinline__ bool group_sync_and(int id, int count, bool pred)
+{
+    uint32_t all;
+    if(id == 1)
+        asm volatile("{ .reg .pred p, q; setp.ne.u32 p, %1, 0; bar.red.and.pred q, 1, %2, p; selp.u32 %0, 1, 0, q; }"
+            : "=r"(all) : "r"(uint32_t(pred)), "r"(count) : "memory");
+    else
+        asm volatile("{ .reg .pred p, q; setp.ne.u32 p, %1, 0; bar.red.and.pred q, 2, %2, p; selp.u32 %0, 1, 0, q; }"
+            : "=r"(all) : "r"(uint32_t(pred)), "r"(count) : "memory");
+    return all != 0u;
+}
+
+// Whether v survives the 16-bit window unchanged: v = s/32768 for an integer s in [-32768, 32767].
+__device__ __forceinline__ bool exact16(float v)
+{
+    const float s = v*32768.0f;
+    return s == rintf(s) && s >= -32768.0f && s <= 32767.0f;
+}
+
 __device__ __forceinline__ void prefetch_l2(const void *p)
 { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 
@@ -724,8 +744,9 @@ __device__ __forceinline__ bool gather_span(const MixParams &P, const BufferRec 
 }
 
 // 16-bit window for the bsinc resamplers.
-// u8/i16/mu-law/A-law samples are exact multiples of 2^-15, so the window can be re-stored as
-// biased 16-bit integers y = 32768*s + 32768 without loss.  Two copies (A: pairs (y0,y1),(y2,y3)..;
+// u8/i16/mu-law/A-law samples are exact multiples of 2^-15, so a window of such samples (its
+// history included, see exact16) can be re-stored as biased 16-bit integers y = 32768*s + 32768
+// without loss.  Two copies (A: pairs (y0,y1),(y2,y3)..;
 // B: pairs (y1,y2),(y3,y4)..) give every window position an aligned pair, so ONE 32-bit shared
 // load feeds two taps: the resampler is bound by shared-memory wavefronts (3 per lane-tap: F, D,
 // sample) and this removes half of the sample loads and their bank conflicts at pitch > 1.
@@ -1182,7 +1203,11 @@ k_mix_voices(const MixParams P)
                 srcDelay = uint32_t(-intPos);
                 if(srcDelay >= srcn) silent = true;
             }
-            group_sync(bar, GS);           // window history in place / previous chunk consumed
+            // window history in place / previous chunk consumed.  The history (win[0, kEdge): mPrevSamples
+            // or the previous chunk's tail, each float written by its own thread) may come from a float
+            // format even when the span after it is 16-bit (a queue of mixed types, a buffer re-pointed
+            // without a reset): the window is packed only when the history is exact in 16 bits too.
+            const bool histExact = group_sync_and(bar, GS, t >= kEdge || exact16(S.win[t]));
             if(silent)
             {
                 for(uint32_t k = t;k < dstn;k += GS) xs[loaded+k] = 0.0f;
@@ -1193,7 +1218,7 @@ k_mix_voices(const MixParams P)
                 float *srcBuffer = S.win + kEdge;
                 bool winInt = false;       // every sample of this window came from a <=16-bit format
                 // the bsinc resamplers read the 16-bit copies when every sample is exact in them
-                const bool pack = resampler >= 4u && !(increment == 65536u && fracPos == 0u);
+                const bool pack = resampler >= 4u && !(increment == 65536u && fracPos == 0u) && histExact;
                 if(!haveBuffer) hold_end_sample<GS>(srcBuffer, srcn, t, bar);
                 else
                 {
