@@ -42,6 +42,16 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
 __device__ __forceinline__ void fence_proxy_async_smem()
 { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---- programmatic dependent launch --------------------------------------------------------
+// Blocks until every grid this one depends on has completed and its memory is visible; returns
+// at once when the grid was launched without the programmatic-serialization attribute.
+__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+// Lets the next grid on the stream (launched with the attribute) be scheduled once every CTA of
+// this grid has executed it or exited.  It counts per CTA: the first thread of a CTA to run it
+// marks the whole CTA, later executions in that CTA are no-ops.
+__device__ __forceinline__ void griddep_launch_dependents()
+{ asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ---- wgmma: Hopper's warpgroup MMA (4 warps issue together, accumulators in registers) ----
 // Shared-memory matrix descriptor (cute::GmmaDescriptor), no swizzle ("interleave"):
 // start address, leading / stride byte offsets (all >> 4), layout type 0.

@@ -2,7 +2,7 @@
 //
 // Owns the device-resident mirrors of the reference's mixer state (voices, buffers,
 // mix buffers, HRTF accumulator carry) and issues the per-update launch sequence:
-//   [k_apply_updates]  k_mix_voices  k_reduce_rows  post-process  (D2H)
+//   [k_apply_updates]  k_mix_voices  [k_hrtf_fir]  k_reduce_rows / post-process  (D2H)
 // on one CUDA stream.  No CPU mixing path exists: every entry point fails with
 // B200MIX_ERR_CUDA when the CUDA runtime/device is unusable.
 #include "../../include/b200mix.h"
@@ -69,7 +69,7 @@ struct b200mix_device {
     DevArray<float> d_dry, d_wet;
     float *d_real{nullptr};                       // d_dry, or inside d_outblock
     DevArray<float> d_partial; size_t partial_floats{0};
-    DevArray<float> d_accum_sum;                  // [2][kAccumLen]
+    uint32_t fir_rows{0};                         // partial rows the last update's HRIR FIR stored
     DevArray<float> d_carry[2];                   // [2][kHrirLen] ping-pong
     int carry_idx{0};
     float *h_real{nullptr};                       // pinned [real][1024]
@@ -206,6 +206,7 @@ struct b200mix_device {
     uint32_t reverb_seq{0};          // update counter of k_reverb_process' early/late hand-off (24 bits used)
     DevArray<uint32_t> d_claim;      // voice claim counters of the parking k_mix_voices
     int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
+    uint64_t fir_done{0};            // `launches` once the last update's k_hrtf_fir was launched
 
     // callback buffers (b200mix_buffer_callback): the registrations (plan slots), the host's
     // mirror of the voices that play them (positions advance by the same arithmetic as on the
@@ -263,6 +264,26 @@ FirVariant get_fir(uint32_t ir_size)
     if(ir_size <= 64u)
         return FirVariant{k_hrtf_fir<17, 64>, sizeof(FirSmem<kFirGS, 17, 64>)*kFirGroups};
     return FirVariant{k_hrtf_fir<19, 128>, sizeof(FirSmem<kFirGS, 19, 128>)*kFirGroups};
+}
+
+static_assert(kPostMaxDry == B200MIX_MAX_DRY_CHANNELS, "k_post_hrtf_reduce: one thread per dry channel");
+
+// Launches fn on the device's stream.  `programmatic`: the kernel directly follows the one it
+// depends on, and may be scheduled once every CTA of that one has executed
+// griddepcontrol.launch_dependents; it must run griddepcontrol.wait before it reads anything
+// that kernel writes.
+template<typename... Args>
+cudaError_t launch_ex(b200mix_device *d, bool programmatic, void (*fn)(Args...), dim3 grid, dim3 block,
+    size_t smem, Args... args)
+{
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = d->stream;
+    cfg.attrs = programmatic ? &attr : nullptr; cfg.numAttrs = programmatic ? 1u : 0u;
+    ++d->launches;
+    return cudaLaunchKernelEx(&cfg, fn, args...);
 }
 
 constexpr uint32_t kDryChunksMax = 128;
@@ -506,7 +527,6 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         d->partial_floats = hrtfDev ? size_t(d->num_sms)*d->fir_blocks_per_sm*(2*kAccumLen)
             : size_t(d->num_sms)*d->mix_blocks_per_sm*size_t(d->mix_cdr)*kLine;
         CUDA_TRY(d, d->d_partial.alloc(std::max<size_t>((hrtfDev ? 1 : 2)*d->partial_floats, 4), d->stream));
-        CUDA_TRY(d, d->d_accum_sum.alloc(2*kAccumLen, d->stream));
         CUDA_TRY(d, d->d_carry[0].alloc(2*kHrirLen, d->stream));
         CUDA_TRY(d, d->d_carry[1].alloc(2*kHrirLen, d->stream));
         CUDA_TRY(d, d->d_temp.alloc(size_t(std::max(dd.dry_channels, 1u))*kLine, d->stream));
@@ -1993,6 +2013,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     d->mix_fn<<<blocks, kMixGS*kMixGroups, d->mix_smem, d->stream>>>(P);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
+    const uint64_t mixDone = d->launches;
 
     stage_mark(d, 2);
     // ---- voices with an active direct filter: filter the parked lines, then mix them ----
@@ -2022,26 +2043,22 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
         }
         CUDA_TRY(d, cudaGetLastError());
     }
-    uint32_t firBlocks = 0;
+    // the HRIR FIR's partial rows are summed by the HRTF post-process (k_post_hrtf_reduce)
+    d->fir_rows = 0;
     if(hrtfDev)
     {
         const FirVariant fir = get_fir(dd.ir_size);
-        firBlocks = std::max(1u, std::min(uint32_t(d->num_sms*d->fir_blocks_per_sm),
+        d->fir_rows = std::max(1u, std::min(uint32_t(d->num_sms*d->fir_blocks_per_sm),
             (d->num_order + kFirGroups - 1)/kFirGroups));
-        fir.fn<<<firBlocks, kFirGS*kFirGroups, fir.smem, d->stream>>>(P);
-        ++d->launches;
-        CUDA_TRY(d, cudaGetLastError());
+        // straight behind the resample kernel (no direct filters in between), its set-up runs
+        // under the resample kernel's last CTAs
+        CUDA_TRY(d, launch_ex(d, d->launches == mixDone, fir.fn, dim3(d->fir_rows), dim3(kFirGS*kFirGroups),
+            fir.smem, P));
+        d->fir_done = d->launches;
     }
     if(d->profile) { cudaEventRecord(d->ev_mix1, d->stream); d->ev_valid = true; }
 
     stage_mark(d, 3);
-    if(hrtfDev)
-    {
-        const uint32_t len = 2*kAccumLen;
-        k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, d->stream>>>(d->d_partial, firBlocks, len,
-            d->d_accum_sum, 0);
-        ++d->launches;
-    }
     if(d->mix_cdr > 0)
     {
         const uint32_t len = uint32_t(d->mix_cdr)*kLine;
@@ -2276,7 +2293,7 @@ static int render_phase_b(b200mix_device *d, uint32_t frames)
     case B200MIX_POST_HRTF:
     {
         PostHrtfParams Q{};
-        Q.accum_sum = d->d_accum_sum; Q.carry_in = d->d_carry[d->carry_idx];
+        Q.partial = d->d_partial; Q.rows = d->fir_rows; Q.carry_in = d->d_carry[d->carry_idx];
         Q.carry_out = d->d_carry[d->carry_idx^1];
         Q.dry = d->d_dry; Q.real = d->d_real; Q.dec_coef = d->d_dec_coef;
         Q.dec_hfscale = d->d_dec_hfscale; Q.dec_state = d->d_dec_state; Q.temp = d->d_temp;
@@ -2288,8 +2305,10 @@ static int render_phase_b(b200mix_device *d, uint32_t frames)
             ++d->launches;
         }
         Q.overwrite = d->real_overwrite ? 1u : 0u;
-        k_post_hrtf_mix<<<dim3((frames + kHrirLen + 127)/128, 2), 128, 0, d->stream>>>(Q);
-        ++d->launches;
+        // straight behind the HRIR FIR (no kernel of the dry bus, sends, effects or band split in
+        // between), it is scheduled under the FIR's last CTAs
+        CUDA_TRY(d, launch_ex(d, d->launches == d->fir_done, k_post_hrtf_reduce,
+            dim3((frames + kHrirLen + kPostTile - 1)/kPostTile, 2), dim3(1024), 0, Q));
         d->carry_idx ^= 1;
         break;
     }
@@ -2394,6 +2413,7 @@ static int shard_wet_exchange(b200mix_device *d)
     {
         if(S.allreduce(d->d_wet, d->d_wet, wetFloats, 7 /*ncclFloat*/, 0 /*ncclSum*/, S.comm, d->stream) != 0)
         { d->error = "ncclAllReduce of the wet buffers failed"; return B200MIX_ERR_CUDA; }
+        d->fir_done = 0;            // a kernel that `launches` does not count
     }
     else
     {
@@ -2749,6 +2769,7 @@ int b200mix_render_begin(b200mix_device *d, uint32_t frames, float **wet_dev, si
     { d->error = "render_begin: a sharded device set exchanges its wet buffers itself — use b200mix_render"; return B200MIX_ERR_INVALID; }
     if(int rc = render_phase_a(d, frames, true, true)) return rc;
     d->mid_render = true; d->mid_frames = frames;
+    d->fir_done = 0;                // the caller may use the stream before render_end
     if(wet_dev) *wet_dev = d->d_wet;
     if(wet_floats) *wet_floats = d->d_wet ? size_t(d->desc.max_slots)*d->desc.wet_channels*kLine : 0;
     return B200MIX_OK;

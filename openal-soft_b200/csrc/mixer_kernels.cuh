@@ -14,8 +14,9 @@
 //      inputs (DoHrtfMix, core/voice.cpp:827-902; MixHrtfBlend/MixHrtf, hrtfbase.h:17-89)
 //      and runs the HRIR FIR with the outputs held in registers ACROSS all voices of the
 //      group (the cross-voice reduction of `Accum[i+j] += ...` happens in registers),
-// and the accumulating kernels store one partial row per CTA; k_reduce_* sums the rows in a
-// fixed order (deterministic output).
+// and the accumulating kernels store one partial row per CTA; k_reduce_* (for the HRIR FIR's
+// rows: k_post_hrtf_reduce, with the HRTF post-mix) sums the rows in a fixed order
+// (deterministic output).
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -1269,6 +1270,13 @@ k_mix_voices(const MixParams P)
     }
 
     if constexpr(CDR > 0) store_partial_row<GS, GROUPS, CDR>(accD, smem_raw, P.partial, g, t);
+    else
+    {
+        // both groups found the claims exhausted: the HRIR FIR may be scheduled (it waits for
+        // this grid's completion before it reads anything the voices wrote)
+        __syncthreads();
+        griddep_launch_dependents();
+    }
 }
 
 // ---------------------------------------------------------------------------
@@ -1326,7 +1334,7 @@ k_mix_deferred(const MixParams P)
 // and runs the HRIR FIR in gather form with OPT contiguous outputs per thread held in
 // registers ACROSS all voices of the group (the cross-voice reduction of `Accum[i+j] += ...`
 // happens in registers, not memory).  Voices are assigned statically in the mixing order and
-// each CTA stores one partial row; k_reduce_rows sums the rows in a fixed order
+// each CTA stores one partial row; k_post_hrtf_reduce sums the rows in a fixed order
 // (deterministic output).  A group's inputs for its next voice are bulk-copied into its second
 // stage buffer while the current voice is built and filtered.
 //   OPT/FP : FIR outputs per thread / front pad (17/64 for ir<=64, 19/128 for ir<=128)
@@ -1387,6 +1395,9 @@ k_hrtf_fir(const MixParams P)
     for(int i = FP + int(n) + t;i < Smem::kLLen;i += GS) S.lLR[i] = make_float2(0.0f, 0.0f);
     if(t == 0) { mbar_init(&S.bar[0], 1u); mbar_init(&S.bar[1], 1u); mbar_fence_init(); }
     group_sync(bar, GS);
+    // launched right behind the resample kernel, the set-up above ran under its tail: what it
+    // writes (sendinfo, the parked lines, the voice records) is read only from here on
+    griddep_wait();
 
     const uint32_t stride = gridDim.x*GROUPS;
     uint32_t v = 0u, info = 0u;
@@ -1495,9 +1506,10 @@ k_hrtf_fir(const MixParams P)
     }
 
     // ---- one partial row per CTA: the groups' register accumulators are summed through
-    //      shared memory in group order (deterministic), halving the rows k_reduce_rows reads
+    //      shared memory in group order (deterministic), halving the rows k_post_hrtf_reduce reads
     const size_t row = blockIdx.x;
     __syncthreads();                         // every group is done with its voice storage
+    griddep_launch_dependents();             // the post-process may be scheduled (it waits for the rows)
     float *stage = reinterpret_cast<float*>(smem_raw);     // >= 2*kAccumLen floats (group 0's area)
     for(int gg = 0;gg < GROUPS;++gg)
     {
@@ -1529,34 +1541,33 @@ k_hrtf_fir(const MixParams P)
 // from L2 at once; the 128 segment sums are then combined in shared memory, 4 at a time in
 // fixed order.  Deterministic: the summation tree depends only on (rows, len).
 constexpr int kReduceCols = 8, kReduceSegs = 128;
-__global__ void __launch_bounds__(1024)
-k_reduce_rows(const float *__restrict__ partial, uint32_t rows, uint32_t len,
-    float *__restrict__ out, int accumulate)
+
+// The CTA's part of that sum: float4 column e4 of the rows (thread col = threadIdx.x % 8 of a
+// 1024-thread CTA), summed when `live`.  Every thread of the CTA calls it; the total is
+// returned to the 8 threads of segment 0 (threadIdx.x < 8).
+__device__ __forceinline__ float4 reduce_rows_cta(const float *__restrict__ partial, uint32_t rows,
+    uint32_t len, uint32_t e4, bool live, float4 (&sm)[kReduceSegs][kReduceCols])
 {
-    __shared__ float4 sm[kReduceSegs][kReduceCols];
     const uint32_t col = threadIdx.x & (kReduceCols-1), seg = threadIdx.x / kReduceCols;
-    const uint32_t e4 = blockIdx.x*kReduceCols + col;
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    if(e4*4u < len)
+    if(live)
     {
         const uint32_t per = (rows + kReduceSegs - 1u)/kReduceSegs;
         const uint32_t r0 = seg*per, r1 = (r0 + per < rows) ? r0 + per : rows;
         const float4 *p = reinterpret_cast<const float4*>(partial) + e4;
         const size_t stride4 = len/4u;
-        uint32_t r = r0;
-        for(;r + 4u <= r1;r += 4u)
+        // up to 8 rows' loads in flight at once (one L2 round trip for a segment of <= 8 rows,
+        // e.g. 528 FIR rows), then added in row order
+        constexpr uint32_t kBatch = 8;
+        for(uint32_t r = r0;r < r1;r += kBatch)
         {
-            const float4 a = __ldg(p + size_t(r)*stride4), b = __ldg(p + size_t(r+1)*stride4);
-            const float4 c = __ldg(p + size_t(r+2)*stride4), d = __ldg(p + size_t(r+3)*stride4);
-            s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
-            s.x += b.x; s.y += b.y; s.z += b.z; s.w += b.w;
-            s.x += c.x; s.y += c.y; s.z += c.z; s.w += c.w;
-            s.x += d.x; s.y += d.y; s.z += d.z; s.w += d.w;
-        }
-        for(;r < r1;++r)
-        {
-            const float4 a = __ldg(p + size_t(r)*stride4);
-            s.x += a.x; s.y += a.y; s.z += a.z; s.w += a.w;
+            float4 a[kBatch];
+            #pragma unroll
+            for(uint32_t k = 0;k < kBatch;++k)
+                if(r + k < r1) a[k] = __ldg(p + size_t(r + k)*stride4);
+            #pragma unroll
+            for(uint32_t k = 0;k < kBatch;++k)
+                if(r + k < r1) { s.x += a[k].x; s.y += a[k].y; s.z += a[k].z; s.w += a[k].w; }
         }
     }
     sm[seg][col] = s;
@@ -1582,11 +1593,25 @@ k_reduce_rows(const float *__restrict__ partial, uint32_t rows, uint32_t len,
         __syncthreads();
         if(width == 2u) break;
     }
-    if(seg == 0 && e4*4u < len)
+    float4 tot = make_float4(0.f, 0.f, 0.f, 0.f);
+    if(seg == 0)
     {
-        float4 tot = sm[0][col];
+        tot = sm[0][col];
         const float4 b = sm[1][col];
         tot.x += b.x; tot.y += b.y; tot.z += b.z; tot.w += b.w;
+    }
+    return tot;
+}
+
+__global__ void __launch_bounds__(1024)
+k_reduce_rows(const float *__restrict__ partial, uint32_t rows, uint32_t len,
+    float *__restrict__ out, int accumulate)
+{
+    __shared__ float4 sm[kReduceSegs][kReduceCols];
+    const uint32_t e4 = blockIdx.x*kReduceCols + (threadIdx.x & (kReduceCols-1));
+    float4 tot = reduce_rows_cta(partial, rows, len, e4, e4*4u < len, sm);
+    if(threadIdx.x < kReduceCols && e4*4u < len)
+    {
         float4 *o = reinterpret_cast<float4*>(out) + e4;
         if(accumulate)
         {
@@ -1889,7 +1914,8 @@ __global__ void __launch_bounds__(64) k_apply_updates(const ApplyParams A)
 // Post-process for HRTF output (DeviceBase::Process(HrtfPostProcess), alc/alu.cpp:289-298
 // -> MixDirectHrtfBase, hrtfbase.h:91-133).
 struct PostHrtfParams {
-    const float *accum_sum;      // [2][kAccumLen] this update's voice contributions
+    const float *partial;        // [rows][2][kAccumLen] the HRIR FIR's partial rows
+    uint32_t rows;
     const float *carry_in;       // [2][kHrirLen]  accumulator tail from the last update
     float *carry_out;            // [2][kHrirLen]
     const float *dry;            // [cd][1024]
@@ -1952,49 +1978,55 @@ __global__ void __launch_bounds__(32) k_post_hrtf_split(const PostHrtfParams Q)
 
 // Stage 2: total[t] = carry[t] + voices[t] + decoder FIR of the dry channels;
 // RealOut L/R (+)= total[0..n); carry_out = total[n..n+128).
-// grid (tiles of 128 outputs, ear); the channels' input spans and this ear's decoder taps are
-// staged in shared memory one channel at a time, so the FIR runs without global loads.
-__global__ void __launch_bounds__(128) k_post_hrtf_mix(const PostHrtfParams Q)
+// voices[t] is the sum of the HRIR FIR's partial rows, summed here with k_reduce_rows' tree for
+// (rows, 2*kAccumLen), so it is the same float as that kernel would store.  grid (tiles of 32
+// outputs, ear), 1024 threads: the row sum first (8 float4 columns x 128 row segments), then
+// thread (output o = tid % 32, channel c = tid / 32) runs channel c's decoder FIR for output o,
+// and the 32 channel sums are added to the total in channel order.
+constexpr uint32_t kPostTile = kReduceCols*4u, kPostMaxDry = 32u;   // B200MIX_MAX_DRY_CHANNELS
+static_assert(kAccumLen % kPostTile == 0, "a tile lies within one ear's accumulator");
+static_assert(kPostMaxDry*kPostTile <= 1024u, "one thread per (channel, output)");
+__global__ void __launch_bounds__(1024, 1) k_post_hrtf_reduce(const PostHrtfParams Q)
 {
-    __shared__ float xs[128 + kHrirLen];
-    __shared__ float cf[kHrirLen];
+    __shared__ float4 sm[kReduceSegs][kReduceCols];
+    __shared__ float vsum[kPostTile];
+    __shared__ float dsum[kPostMaxDry][kPostTile];
     const uint32_t span = Q.frames + kHrirLen;
     const uint32_t ear = blockIdx.y;
-    const uint32_t t0 = blockIdx.x*128u, tt = t0 + threadIdx.x;
-    float tot = 0.0f;
-    if(tt < span)
+    const uint32_t t0 = blockIdx.x*kPostTile;
+    // the FIR's partial rows (and, launched right behind it, everything it wrote) are complete
+    griddep_wait();
+    const uint32_t col = threadIdx.x & (kReduceCols-1);
+    const uint32_t e4 = (ear*kAccumLen + t0)/4u + col;
+    const float4 v = reduce_rows_cta(Q.partial, Q.rows, 2u*kAccumLen, e4, t0 + 4u*col < span, sm);
+    if(threadIdx.x < kReduceCols)
+    { vsum[4*col] = v.x; vsum[4*col + 1] = v.y; vsum[4*col + 2] = v.z; vsum[4*col + 3] = v.w; }
+
+    const uint32_t o = threadIdx.x % kPostTile, c = threadIdx.x / kPostTile;
+    const uint32_t tt = t0 + o;
+    if(Q.dry_active && c < Q.cd)
     {
-        tot = Q.accum_sum[ear*kAccumLen + tt];
-        if(tt < uint32_t(kHrirLen)) tot += Q.carry_in[ear*kHrirLen + tt];
-    }
-    if(Q.dry_active)
-    {
-        const uint32_t jmax = Q.dec_ir;                // <= kHrirLen
-        for(uint32_t c = 0;c < Q.cd;++c)
+        const float *x = Q.temp + size_t(c)*kLine;
+        const float2 *cg = Q.dec_coef + size_t(c)*Q.dec_ir;
+        float s = 0.0f;
+        for(uint32_t j = 0;j < Q.dec_ir;++j)           // dec_ir <= kHrirLen
         {
-            const float *x = Q.temp + size_t(c)*kLine;
-            const float2 *cg = Q.dec_coef + size_t(c)*Q.dec_ir;
-            __syncthreads();
-            // xs[k] = x[t0 - kHrirLen + k], zero outside [0, frames)
-            for(uint32_t k = threadIdx.x;k < 128u + kHrirLen;k += 128u)
-            {
-                const int src = int(t0) - int(kHrirLen) + int(k);
-                xs[k] = (src >= 0 && src < int(Q.frames)) ? x[src] : 0.0f;
-            }
-            if(threadIdx.x < jmax) cf[threadIdx.x] = ear ? cg[threadIdx.x].y : cg[threadIdx.x].x;
-            __syncthreads();
-            float s = 0.0f;
-            const float *w = xs + kHrirLen + threadIdx.x;
-            for(uint32_t j = 0;j < jmax;++j)
-                s = fmaf(cf[j], w[-int(j)], s);
-            tot += s;
+            const int src = int(tt) - int(j);
+            const float xv = (src >= 0 && src < int(Q.frames)) ? x[src] : 0.0f;
+            s = fmaf(ear ? cg[j].y : cg[j].x, xv, s);
         }
+        dsum[c][o] = s;
     }
-    if(tt >= span) return;
+    __syncthreads();
+    if(threadIdx.x >= kPostTile || tt >= span) return;
+    float tot = vsum[o];
+    if(tt < uint32_t(kHrirLen)) tot += Q.carry_in[ear*kHrirLen + tt];
+    if(Q.dry_active)
+        for(uint32_t ch = 0;ch < Q.cd;++ch) tot += dsum[ch][o];
     if(tt < Q.frames)
     {
-        float *o = Q.real + size_t(ear ? Q.real_right : Q.real_left)*kLine + tt;
-        *o = Q.overwrite ? tot : (*o + tot);
+        float *out = Q.real + size_t(ear ? Q.real_right : Q.real_left)*kLine + tt;
+        *out = Q.overwrite ? tot : (*out + tot);
     }
     else
         Q.carry_out[ear*kHrirLen + (tt - Q.frames)] = tot;
