@@ -31,6 +31,7 @@
 #include "adpcm.hpp"
 #include "callback_plan.hpp"
 #include "device_memory.hpp"
+#include "voice_book.hpp"
 
 using namespace b200mix;
 
@@ -56,8 +57,8 @@ struct b200mix_device {
     DevArray<VoiceRec> d_voices; DevArray<BufferRec> d_buffers;
     std::vector<BufferRec> h_buffers;
     std::vector<DevArray<char>> buf_store;       // per buffer: the samples its h_buffers record views
-    std::vector<uint32_t> h_vbuf;                 // static buffer an active voice plays (or NO_SLOT)
-    std::vector<uint32_t> h_bufrefs;              // active static voices per buffer
+    VoiceBook book;                               // host mirror of the voices, source of d_order & co.
+    DevArray<uint32_t> d_order;                   // book.order
     DevArray<float2> d_hrtf_tgt, d_hrtf_old;
     DevArray<float> d_dry_cur, d_dry_tgt, d_send_cur, d_send_tgt;
     VoiceResult *d_results{nullptr};              // inside d_outblock
@@ -80,7 +81,6 @@ struct b200mix_device {
     DevArray<float> d_temp, d_temp2;
     uint32_t amb_in{0}; bool amb_dual{false};
     DevArray<float> d_amb_hf, d_amb_lf, d_amb_state;
-    bool dry_active{false};
     DevArray<float> d_uhj_state, d_uhj_scratch;
     uint32_t stab_center{B200MIX_NO_SLOT};                // StablizerPostProcess: FrontCenter index
     float stab_coeff{0.0f};
@@ -102,17 +102,8 @@ struct b200mix_device {
     DevArray<FilterRec> d_filt;
     UploadArena fstage;                      // b200mix_voices_filters' inputs
     DevArray<float> d_fscratch, d_dline;     // [rows][1024]; [max_voices][1024] filtered direct-path lines
-    std::vector<uint8_t> h_dfilt;            // host mirror: direct filter active per voice
-    std::vector<uint32_t> h_order2;          // active voices with an active direct filter
-    DevArray<uint32_t> d_order2;
-    uint32_t num_order2{0};
-    bool order2_dirty{false};
-    std::vector<uint32_t> h_send_slot;       // [max_voices][MAX_SENDS] host mirror
-    std::vector<uint32_t> h_slot_start;
-    std::vector<SendEntry> h_entries;
-    DevArray<uint32_t> d_slot_start; DevArray<SendEntry> d_entries;
-    uint32_t num_entries{0};
-    bool sends_dirty{true};
+    DevArray<uint32_t> d_order2;             // book.order2
+    DevArray<uint32_t> d_slot_start; DevArray<SendEntry> d_entries;   // book.slot_start / book.entries
     // EFX effect slots (b200mix_slot_efx): host mirrors + the per-slot views the kernel walks
     struct EfxHost { bool used{false}; EfxParams p{}; DevArray<EfxDev> dev; uint32_t mod_index{0}, mod_range{1};
         uint32_t lfo_offset{0}, lfo_range{1}; };
@@ -147,17 +138,12 @@ struct b200mix_device {
     bool mid_render{false}; uint32_t mid_frames{0};   // between render_begin and render_end
     bool real_overwrite{false};
     // parked dry bus (kernel variants without register dry accumulators)
-    std::vector<uint8_t> h_hrtf;             // host mirror: voice mixes through its own HRIR
-    std::vector<SendEntry> h_dry_entries;
-    DevArray<SendEntry> d_dry_entries; DevArray<uint32_t> d_dry_slot_start;
-    uint32_t num_dry_entries{0};
-    bool dry_entries_dirty{true};
+    DevArray<SendEntry> d_dry_entries; DevArray<uint32_t> d_dry_slot_start;   // book.dry_entries
     DevArray<float> d_dry_partial;           // [kDryChunksMax][cd][1024]
     DevArray<float> d_dry_geff;              // [max_voices][cd]
     DevArray<float> d_send_geff;             // [max_voices*num_sends][cw]
     DevArray<float4> d_dry_gramp, d_send_gramp;
     DevArray<float> d_send_partial;          // [send_chunks][max_slots][cw][1024]
-    uint32_t max_slot_entries{0};
     bool profile{false};
     Event ev_mix0, ev_mix1;
     bool ev_valid{false};
@@ -166,17 +152,8 @@ struct b200mix_device {
     Event ev_stage[kStages + 1];
     bool stage_valid{false}; int profile_level{0};
 
-    // mixing order (host mirror of which voices are configured active, and their cost)
-    std::vector<uint8_t> h_active;
-    std::vector<uint32_t> h_cost;
-    std::vector<uint32_t> h_order;
-    DevArray<uint32_t> d_order;
-    uint32_t num_order{0};
-    bool order_dirty{true};
-
     // GPU parameter stage (b200mix_sources_update): pinned input staging + device scratch
     UploadArena src;
-    bool dev_filters{false};                 // filter activity is decided on the device: order2 = order
     bool panmix_tc{false};                   // wide dry buses: pan-mix past the fades on the tensor cores
 
     // voice-sharded device set (b200mix_shard_*): transport 0 none, 1 peer stores, 2 NCCL
@@ -199,7 +176,6 @@ struct b200mix_device {
     } shard;
 
     uint32_t ir_pad{0};
-    uint32_t voice_hi{0};          // 1 + highest voice index ever configured
     // resample kernel (resolved at create): k_mix_voices<kMixGS, kMixGroups, mix_cdr>
     void (*mix_fn)(const MixParams){nullptr};
     size_t mix_smem{0}; int mix_cdr{0}; int mix_blocks_per_sm{1};
@@ -375,6 +351,73 @@ const BsincTable *bsinc_for(const b200mix_device *d, uint32_t resampler)
     return &d->bsinc[(resampler - B200MIX_RESAMPLER_FAST_BSINC12) >> 1];
 }
 
+// Plan slot of the callback buffer an entry plays (-1: none).
+int32_t cb_slot_of(const b200mix_device *d, uint32_t flags, uint32_t buffer)
+{
+    return (!(flags & B200MIX_VF_STOPPED) && buffer != B200MIX_NO_BUFFER && !d->cb_of_buffer.empty())
+        ? d->cb_of_buffer[buffer] : -1;
+}
+
+// The checks b200mix_voices_update and b200mix_sources_update make of every entry before the call
+// changes anything; `what` prefixes the error.  They may allocate the queue tables and the parked
+// dry bus, which leave the device as it was if they fail.  `nobuf_ok`: the entry may name
+// B200MIX_NO_BUFFER; `hrtf`: the voice mixes through its own HRIR.
+template<typename Entry>
+int check_entry(b200mix_device *d, const char *what, const Entry &p, bool nobuf_ok, bool hrtf)
+{
+    const b200mix_device_desc &dd = d->desc;
+    const bool stopped = (p.flags & B200MIX_VF_STOPPED) != 0;
+    const bool nobuf = nobuf_ok && p.buffer == B200MIX_NO_BUFFER;
+    auto bad = [&](const char *why) { d->error = std::string(what) + ": " + why; return B200MIX_ERR_INVALID; };
+    if(p.voice >= dd.max_voices || p.resampler > B200MIX_RESAMPLER_BSINC48
+        || (!stopped && !nobuf && p.buffer >= dd.max_buffers))
+        return bad("voice/buffer/resampler out of range");
+    if((p.flags & B200MIX_VF_LOOPING) && p.loop_end <= p.loop_start)
+        return bad("empty loop");
+    // nothing to read without a buffer; a callback voice reads from the update's arena
+    if(!stopped && !nobuf && cb_slot_of(d, p.flags, p.buffer) < 0)
+    {
+        if(p.flags & B200MIX_VF_STATIC)
+        {
+            const BufferRec &hb = d->h_buffers[p.buffer];
+            if(!hb.data || !hb.frames) return bad("static voice on a buffer without data");
+            if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames) return bad("loop end beyond the buffer");
+        }
+        // a streaming voice reads its queue: make sure the (empty) queue table exists
+        else if(int rc = ensure_queues(d)) return rc;
+    }
+    for(uint32_t s = 0;s < dd.num_sends;++s)
+        if(p.send_slot[s] != B200MIX_NO_SLOT && p.send_slot[s] >= dd.max_slots)
+            return bad("send slot out of range");
+    if(!stopped && !hrtf && d->mix_cdr == 0)
+        if(int rc = ensure_dry_park(d)) return rc;
+    return B200MIX_OK;
+}
+
+// k_apply_updates' parameters that do not depend on the entry point.
+ApplyParams apply_params(const b200mix_device *d, const VoiceUpdate *updates)
+{
+    const b200mix_device_desc &dd = d->desc;
+    ApplyParams A{};
+    A.voices = d->d_voices; A.updates = updates;
+    A.hrtf_tgt = d->d_hrtf_tgt; A.hrtf_old = d->d_hrtf_old;
+    A.dry_cur = d->d_dry_cur; A.dry_tgt = d->d_dry_tgt;
+    A.send_cur = d->d_send_cur; A.send_tgt = d->d_send_tgt;
+    A.ir = dd.ir_size; A.ir_pad = d->ir_pad; A.cd = dd.dry_channels; A.cw = dd.wet_channels;
+    A.num_sends = dd.num_sends;
+    A.filt = d->d_filt; A.filt_paths = 1u + dd.num_sends;
+    A.qhdr = d->d_qhdr;
+    return A;
+}
+
+// Entries given as directions: the HRIRs are blended on the device from the attached data set.
+void apply_dirs(const b200mix_device *d, ApplyParams &A, const float4 *dirs)
+{
+    A.dirs = dirs;
+    A.st_fields = d->d_st_fields; A.st_elevs = d->d_st_elevs; A.st_coeffs = d->d_st_coeffs;
+    A.st_delays = d->d_st_delays; A.st_num_fields = d->st_num_fields; A.st_ir = d->st_ir;
+}
+
 } // namespace
 
 extern "C" {
@@ -445,8 +488,7 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         CUDA_TRY(d, d->d_buffers.alloc(std::max(dd.max_buffers, 1u), d->stream));
         d->h_buffers.assign(std::max(dd.max_buffers, 1u), BufferRec{});
         d->buf_store.resize(d->h_buffers.size());
-        d->h_vbuf.assign(dd.max_voices, B200MIX_NO_SLOT);
-        d->h_bufrefs.assign(std::max(dd.max_buffers, 1u), 0u);
+        d->book.init(dd.max_voices, dd.max_buffers, dd.num_sends, dd.max_slots);
         if(dd.ir_size)
         {
             CUDA_TRY(d, d->d_hrtf_tgt.alloc(size_t(dd.max_voices)*d->ir_pad, d->stream));
@@ -461,9 +503,6 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
             CUDA_TRY(d, d->d_send_tgt.alloc(dd.max_voices*per, d->stream));
         }
         CUDA_TRY(d, d->d_order.alloc(dd.max_voices, d->stream));
-        d->h_active.assign(dd.max_voices, 0);
-        d->h_cost.assign(dd.max_voices, 0);
-        d->h_hrtf.assign(dd.max_voices, 0);
 
         // resample kernel: non-HRTF devices with <= 4 dry channels mix the dry bus in registers;
         // HRTF devices and wider dry mixes resample + park (k_hrtf_fir mixes the HRTF voices,
@@ -539,7 +578,6 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
             if(int rc = ensure_park_lines(d)) return rc;
             CUDA_TRY(d, d->d_send_geff.alloc(size_t(dd.max_voices)*dd.num_sends*dd.wet_channels, d->stream));
             CUDA_TRY(d, d->d_send_gramp.alloc(size_t(dd.max_voices)*dd.num_sends*dd.wet_channels, d->stream));
-            d->h_send_slot.assign(size_t(dd.max_voices)*B200MIX_MAX_SENDS, B200MIX_NO_SLOT);
             CUDA_TRY(d, d->d_slot_start.alloc(dd.max_slots + 1, d->stream));
             CUDA_TRY(d, d->d_entries.alloc(size_t(dd.max_voices)*dd.num_sends, d->stream));
             std::vector<float2> tw(128);
@@ -636,7 +674,7 @@ int b200mix_set_ambi_decoder(b200mix_device *d, uint32_t in_channels, const floa
 static uint32_t cb_slot_voices(const b200mix_device *d, int32_t s)
 {
     uint32_t n = 0;
-    for(uint32_t v = 0;v < d->cbv.size() && v < d->voice_hi;++v)
+    for(uint32_t v = 0;v < d->cbv.size() && v < d->book.voice_hi;++v)
         n += d->cbv[v].slot == s && (d->cbv[v].v.state == 1u || d->cbv[v].v.state == 2u);
     return n;
 }
@@ -695,7 +733,7 @@ int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_ca
     int32_t s = d->cb_of_buffer[buffer];
     if(s < 0)
     {
-        if(h.data && d->h_bufrefs[buffer])
+        if(h.data && d->book.bufrefs[buffer])
         { d->error = "buffer_callback: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
         if(h.data)
         {
@@ -746,7 +784,7 @@ int b200mix_buffer_data(b200mix_device *d, uint32_t buffer, uint32_t sample_type
     const size_t need = size_t(frames)*channels*sz[sample_type];
     if(bytes < need) { d->error = "buffer_data: short data"; return B200MIX_ERR_INVALID; }
     BufferRec &h = d->h_buffers[buffer];
-    if(h.data && d->h_bufrefs[buffer])
+    if(h.data && d->book.bufrefs[buffer])
     { d->error = "buffer_data: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
     DevArray<char> &store = d->buf_store[buffer];
     if(h.data)
@@ -791,7 +829,7 @@ int b200mix_buffer_free(b200mix_device *d, uint32_t buffer)
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     if(int rc = cb_unregister(d, buffer, "buffer_free")) return rc;
     BufferRec &h = d->h_buffers[buffer];
-    if(h.data && d->h_bufrefs[buffer])
+    if(h.data && d->book.bufrefs[buffer])
     { d->error = "buffer_free: the buffer is attached to an active voice; stop the voice first"; return B200MIX_ERR_INVALID; }
     if(h.data)
     {
@@ -934,7 +972,7 @@ int b200mix_slot_convolution(b200mix_device *d, uint32_t slot, uint32_t ir_chann
     CUDA_TRY(d, cudaMemcpyAsync(d->d_slots + slot, &d->h_slots[slot], sizeof(SlotRec), cudaMemcpyHostToDevice, d->stream));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     ++d->active_slots;
-    d->dry_active = true;
+    d->book.dry_active = true;
     return update_stages(d);
 }
 
@@ -1057,7 +1095,7 @@ int b200mix_slot_reverb(b200mix_device *d, uint32_t slot, const b200mix_reverb_p
     CUDA_TRY(d, cudaMemcpyAsync(d->d_slots + slot, &d->h_slots[slot], sizeof(SlotRec), cudaMemcpyHostToDevice, d->stream));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     ++d->active_slots; ++d->reverb_slots;
-    d->dry_active = true;
+    d->book.dry_active = true;
     return update_stages(d);
 }
 
@@ -1126,7 +1164,7 @@ int b200mix_slot_efx(b200mix_device *d, uint32_t slot, const b200mix_efx_props *
         d->h_slots[slot] = r;
         ++d->active_slots; ++d->efx_slots;
         if(props->type == B200MIX_EFFECT_PSHIFTER) ++d->pshift_slots;
-        d->dry_active = true;
+        d->book.dry_active = true;
     }
     else
     {
@@ -1291,7 +1329,7 @@ static int cb_group(b200mix_device *d)
     reps.assign(d->cbs.size(), -1);
     d->cb_members.resize(d->cbs.size());
     for(auto &m : d->cb_members) m.clear();
-    for(uint32_t v = 0;v < d->voice_hi;++v)
+    for(uint32_t v = 0;v < d->book.voice_hi;++v)
     {
         const b200mix_device::CbVoice &cv = d->cbv[v];
         if(cv.slot < 0 || (cv.v.state != 1u && cv.v.state != 2u)) continue;
@@ -1332,45 +1370,34 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     if(!params) { d->error = "voices_update: null params"; return B200MIX_ERR_INVALID; }
     const b200mix_device_desc &dd = d->desc;
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    CUDA_TRY(d, d->stage.wait());
-    if(int rc = ensure_stage(d, n)) return rc;
-    d->stage.begin();
-    VoiceUpdate *const upd = d->stage.host_part<VoiceUpdate>(n);
-
     for(uint32_t i = 0;i < n;++i)
     {
         const b200mix_voice_params &p = params[i];
-        const bool nobuf = p.buffer == B200MIX_NO_BUFFER;
-        if(p.voice >= dd.max_voices || p.resampler > B200MIX_RESAMPLER_BSINC48
-            || (!(p.flags & B200MIX_VF_STOPPED) && !nobuf && p.buffer >= dd.max_buffers))
-        { d->error = "voices_update: voice/buffer/resampler out of range"; return B200MIX_ERR_INVALID; }
-        if((p.flags & B200MIX_VF_LOOPING) && p.loop_end <= p.loop_start)
-        { d->error = "voices_update: empty loop"; return B200MIX_ERR_INVALID; }
+        if(int rc = check_entry(d, "voices_update", p, true, (p.flags & B200MIX_VF_HRTF) != 0)) return rc;
         // MaxPitch clamp of the parameter stage (alc/alu.cpp:1682-1685,1996-1999): CalculateBufferSize
         // relies on it
         if(p.step > (10u << 16))
         { d->error = "voices_update: step above MaxPitch<<16"; return B200MIX_ERR_INVALID; }
+        // with directions the delays are computed on the device
+        if(!dirs && (p.hrtf_delay[0] >= B200MIX_HRTF_HISTORY || p.hrtf_delay[1] >= B200MIX_HRTF_HISTORY))
+        { d->error = "voices_update: HRTF delay out of range"; return B200MIX_ERR_INVALID; }
         // callback voice: plays a buffer made by b200mix_buffer_callback
-        const int32_t cbSlot = (!(p.flags & B200MIX_VF_STOPPED) && !nobuf && !d->cb_of_buffer.empty())
-            ? d->cb_of_buffer[p.buffer] : -1;
+        const int32_t cbSlot = cb_slot_of(d, p.flags, p.buffer);
         if(cbSlot >= 0 && (p.flags & B200MIX_VF_STATIC))
         { d->error = "voices_update: a callback buffer is not static (IsCallback)"; return B200MIX_ERR_INVALID; }
         if(cbSlot >= 0 && d->cbv[p.voice].slot != cbSlot && !(p.flags & B200MIX_VF_RESET))
         { d->error = "voices_update: a voice starts a callback buffer with B200MIX_VF_RESET"; return B200MIX_ERR_INVALID; }
-        if(!(p.flags & B200MIX_VF_STOPPED))
-        {
-            if(nobuf || cbSlot >= 0) { /* nothing to read / read from the update's arena */ }
-            else if(p.flags & B200MIX_VF_STATIC)
-            {
-                const BufferRec &hb = d->h_buffers[p.buffer];
-                if(!hb.data || !hb.frames)
-                { d->error = "voices_update: static voice on a buffer without data"; return B200MIX_ERR_INVALID; }
-                if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames)
-                { d->error = "voices_update: loop end beyond the buffer"; return B200MIX_ERR_INVALID; }
-            }
-            // a streaming voice reads its queue: make sure the (empty) queue table exists
-            else if(int rc = ensure_queues(d)) return rc;
-        }
+    }
+
+    CUDA_TRY(d, d->stage.wait());
+    if(int rc = ensure_stage(d, n)) return rc;
+    d->stage.begin();
+    VoiceUpdate *const upd = d->stage.host_part<VoiceUpdate>(n);
+    for(uint32_t i = 0;i < n;++i)
+    {
+        const b200mix_voice_params &p = params[i];
+        const bool nobuf = p.buffer == B200MIX_NO_BUFFER;
+        const bool stopped = (p.flags & B200MIX_VF_STOPPED) != 0;
         VoiceUpdate &u = upd[i];
         u.voice = p.voice; u.flags = p.flags; u.buffer = p.buffer; u.resampler = p.resampler;
         if(nobuf) { u.flags |= kUpNoBuffer; u.buffer = 0u; }
@@ -1382,48 +1409,20 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
             const BsincState st = PrepareBsinc(*t, p.step);
             u.bsinc_sf = st.sf; u.bsinc_m = st.m; u.bsinc_l = st.l; u.bsinc_off = st.offset;
         }
-        u.delay0 = p.hrtf_delay[0]; u.delay1 = p.hrtf_delay[1]; u.gain = p.hrtf_gain;
-        if(dirs) { u.delay0 = 0; u.delay1 = 0; }        // computed on the device
-        if(u.delay0 >= B200MIX_HRTF_HISTORY || u.delay1 >= B200MIX_HRTF_HISTORY)
-        { d->error = "voices_update: HRTF delay out of range"; return B200MIX_ERR_INVALID; }
+        u.delay0 = dirs ? 0 : p.hrtf_delay[0]; u.delay1 = dirs ? 0 : p.hrtf_delay[1]; u.gain = p.hrtf_gain;
         for(uint32_t s = 0;s < B200MIX_MAX_SENDS;++s)
-        {
             u.send_slot[s] = (s < dd.num_sends) ? p.send_slot[s] : B200MIX_NO_SLOT;
-            if(u.send_slot[s] != B200MIX_NO_SLOT && u.send_slot[s] >= dd.max_slots)
-            { d->error = "voices_update: send slot out of range"; return B200MIX_ERR_INVALID; }
-        }
-        if(!d->h_send_slot.empty())
-            for(uint32_t s2 = 0;s2 < B200MIX_MAX_SENDS;++s2)
-            {
-                uint32_t &m = d->h_send_slot[size_t(p.voice)*B200MIX_MAX_SENDS + s2];
-                const uint32_t nv2 = (p.flags & B200MIX_VF_STOPPED) ? B200MIX_NO_SLOT : u.send_slot[s2];
-                if(m != nv2) { m = nv2; d->sends_dirty = true; }
-            }
         u.has_coeffs = (hrtf_coeffs != nullptr || (dirs != nullptr && (p.flags & B200MIX_VF_HRTF))) && dd.ir_size > 0;
         u.has_dry = dry_gains != nullptr;
-        if(!(p.flags & B200MIX_VF_HRTF) && !(p.flags & B200MIX_VF_STOPPED))
-        {
-            d->dry_active = true;
-            if(d->mix_cdr == 0)
-                if(int rc = ensure_dry_park(d)) return rc;
-        }
-        {
-            const uint8_t hv = (p.flags & B200MIX_VF_HRTF) ? 1 : 0;
-            if(d->h_hrtf[p.voice] != hv) { d->h_hrtf[p.voice] = hv; d->dry_entries_dirty = true; }
-        }
-        {
-            // mixing-order bookkeeping: membership and a cost key (resampler taps per output)
-            const uint8_t act = (p.flags & B200MIX_VF_STOPPED) ? 0 : 1;
-            uint32_t cost = (p.step == 65536u) ? 1u : (u.bsinc_m ? u.bsinc_m : (p.resampler >= 2u ? 4u : 2u));
-            if(d->h_active[p.voice] != act || d->h_cost[p.voice] != cost) d->order_dirty = true;
-            d->h_active[p.voice] = act; d->h_cost[p.voice] = cost;
-        }
-        d->voice_hi = std::max(d->voice_hi, p.voice + 1u);
+        // mixing-order cost key: resampler taps per output
+        const uint32_t cost = (p.step == 65536u) ? 1u : (u.bsinc_m ? u.bsinc_m : (p.resampler >= 2u ? 4u : 2u));
+        d->book.set(p.voice, {!stopped, cost, (p.flags & B200MIX_VF_HRTF) != 0, p.send_slot,
+            (p.flags & B200MIX_VF_STATIC) && !nobuf ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0});
         if(!d->cbv.empty())
         {
             // the planner's mirror of the voice: what k_apply_updates does to its record
             b200mix_device::CbVoice &cv = d->cbv[p.voice];
-            const int32_t slot = nobuf && !(p.flags & B200MIX_VF_STOPPED) ? cv.slot : cbSlot;
+            const int32_t slot = nobuf && !stopped ? cv.slot : cb_slot_of(d, p.flags, p.buffer);
             if(slot != cv.slot)
             {
                 d->cb_bound = d->cb_bound + (slot >= 0) - (cv.slot >= 0);
@@ -1443,31 +1442,13 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
                 if(nobuf) m.have_buffer = false;
             }
         }
-        {
-            const uint32_t nb = (!(p.flags & B200MIX_VF_STOPPED) && (p.flags & B200MIX_VF_STATIC) && !nobuf)
-                ? p.buffer : B200MIX_NO_SLOT;
-            uint32_t &ob = d->h_vbuf[p.voice];
-            if(ob != nb)
-            {
-                if(ob != B200MIX_NO_SLOT) --d->h_bufrefs[ob];
-                if(nb != B200MIX_NO_SLOT) ++d->h_bufrefs[nb];
-                ob = nb;
-            }
-        }
-        if((p.flags & B200MIX_VF_RESET) && !d->h_dfilt.empty() && d->h_dfilt[p.voice])
-        { d->h_dfilt[p.voice] = 0; d->order2_dirty = true; }
     }
     if(d->cb_bound)
         if(int rc = cb_group(d)) return rc;
-    ApplyParams A{};
-    A.voices = d->d_voices; A.updates = d->stage.dev_of(upd);
+    ApplyParams A = apply_params(d, d->stage.dev_of(upd));
     auto pack = [d](const float *src, size_t count) { return d->stage.pack(src, count); };
     if(dirs && dd.ir_size)
-    {
-        A.dirs = reinterpret_cast<const float4*>(pack(dirs, size_t(n)*4));
-        A.st_fields = d->d_st_fields; A.st_elevs = d->d_st_elevs; A.st_coeffs = d->d_st_coeffs;
-        A.st_delays = d->d_st_delays; A.st_num_fields = d->st_num_fields; A.st_ir = d->st_ir;
-    }
+        apply_dirs(d, A, reinterpret_cast<const float4*>(pack(dirs, size_t(n)*4)));
     else if(hrtf_coeffs && dd.ir_size)
         A.coeffs = pack(hrtf_coeffs, size_t(n)*dd.ir_size*2);
     if(dry_gains && dd.dry_channels)
@@ -1475,13 +1456,6 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     if(send_gains && dd.num_sends && dd.wet_channels)
         A.send = pack(send_gains, size_t(n)*dd.num_sends*dd.wet_channels);
     CUDA_TRY(d, d->stage.ship(d->stream));
-    A.hrtf_tgt = d->d_hrtf_tgt; A.hrtf_old = d->d_hrtf_old;
-    A.dry_cur = d->d_dry_cur; A.dry_tgt = d->d_dry_tgt;
-    A.send_cur = d->d_send_cur; A.send_tgt = d->d_send_tgt;
-    A.ir = dd.ir_size; A.ir_pad = d->ir_pad; A.cd = dd.dry_channels; A.cw = dd.wet_channels;
-    A.num_sends = dd.num_sends;
-    A.filt = d->d_filt; A.filt_paths = 1u + dd.num_sends;
-    A.qhdr = d->d_qhdr;
     k_apply_updates<<<n, 64, 0, d->stream>>>(A);
     ++d->launches;
     CUDA_TRY(d, cudaGetLastError());
@@ -1530,80 +1504,15 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
         const b200mix_source_props &P = props[i];
         if(P.struct_size != sizeof(P) || P.distance_model > 6u)
         { d->error = "sources_update: bad source props"; return B200MIX_ERR_INVALID; }
-        if(p.voice >= dd.max_voices || p.resampler > B200MIX_RESAMPLER_BSINC48
-            || (!(p.flags & B200MIX_VF_STOPPED) && p.buffer >= dd.max_buffers))
-        { d->error = "sources_update: voice/buffer/resampler out of range"; return B200MIX_ERR_INVALID; }
-        if((p.flags & B200MIX_VF_LOOPING) && p.loop_end <= p.loop_start)
-        { d->error = "sources_update: empty loop"; return B200MIX_ERR_INVALID; }
+        if(int rc = check_entry(d, "sources_update", p, false, hrtfMode)) return rc;
         // callback voices are planned from the steps b200mix_voices_update gives; this stage
         // computes them on the device, where the planner cannot see them
-        if(!(p.flags & B200MIX_VF_STOPPED) && !d->cb_of_buffer.empty() && d->cb_of_buffer[p.buffer] >= 0)
+        if(cb_slot_of(d, p.flags, p.buffer) >= 0)
         { d->error = "sources_update: callback buffers play through b200mix_voices_update"; return B200MIX_ERR_UNSUPPORTED; }
-        if(!(p.flags & B200MIX_VF_STOPPED))
-        {
-            if(p.flags & B200MIX_VF_STATIC)
-            {
-                const BufferRec &hb = d->h_buffers[p.buffer];
-                if(!hb.data || !hb.frames)
-                { d->error = "sources_update: static voice on a buffer without data"; return B200MIX_ERR_INVALID; }
-                if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames)
-                { d->error = "sources_update: loop end beyond the buffer"; return B200MIX_ERR_INVALID; }
-            }
-            else if(int rc = ensure_queues(d)) return rc;
-        }
-        for(uint32_t s = 0;s < dd.num_sends;++s)
-            if(p.send_slot[s] != B200MIX_NO_SLOT && p.send_slot[s] >= dd.max_slots)
-            { d->error = "sources_update: send slot out of range"; return B200MIX_ERR_INVALID; }
         if(!mayFilter && source_may_filter(P, dd.num_sends)) mayFilter = true;
     }
     if(mayFilter)
-    {
         if(int rc = ensure_filters(d)) return rc;
-        if(!d->dev_filters) { d->dev_filters = true; d->order2_dirty = true; }
-    }
-    // host mirrors (as b200mix_voices_update keeps them); the step is not known here: the cost
-    // key of the mixing order takes the resampler's widest filter
-    for(uint32_t i = 0;i < n;++i)
-    {
-        const b200mix_source_voice &p = voices[i];
-        const bool stopped = (p.flags & B200MIX_VF_STOPPED) != 0;
-        // the voice no longer plays a callback buffer
-        if(!d->cbv.empty() && d->cbv[p.voice].slot >= 0)
-        {
-            d->cbv[p.voice].slot = -1;
-            --d->cb_bound;
-        }
-        if(!d->h_send_slot.empty())
-            for(uint32_t s2 = 0;s2 < B200MIX_MAX_SENDS;++s2)
-            {
-                uint32_t &m = d->h_send_slot[size_t(p.voice)*B200MIX_MAX_SENDS + s2];
-                const uint32_t nv2 = (stopped || s2 >= dd.num_sends) ? B200MIX_NO_SLOT : p.send_slot[s2];
-                if(m != nv2) { m = nv2; d->sends_dirty = true; }
-            }
-        if(!hrtfMode && !stopped)
-        {
-            d->dry_active = true;
-            if(d->mix_cdr == 0)
-                if(int rc = ensure_dry_park(d)) return rc;
-        }
-        const uint8_t hv = hrtfMode ? 1 : 0;
-        if(d->h_hrtf[p.voice] != hv) { d->h_hrtf[p.voice] = hv; d->dry_entries_dirty = true; }
-        const uint8_t act = stopped ? 0 : 1;
-        uint32_t cost = p.resampler >= 2u ? 4u : 2u;
-        if(const BsincTable *t = bsinc_for(d, p.resampler)) cost = t->m[0];
-        if(d->h_active[p.voice] != act || (!d->h_cost[p.voice] && act)) { d->order_dirty = true; d->h_cost[p.voice] = cost; }
-        d->h_active[p.voice] = act;
-        d->voice_hi = std::max(d->voice_hi, p.voice + 1u);
-        const uint32_t nb = (!stopped && (p.flags & B200MIX_VF_STATIC)) ? p.buffer : B200MIX_NO_SLOT;
-        uint32_t &ob = d->h_vbuf[p.voice];
-        if(ob != nb)
-        {
-            if(ob != B200MIX_NO_SLOT) --d->h_bufrefs[ob];
-            if(nb != B200MIX_NO_SLOT) ++d->h_bufrefs[nb];
-            ob = nb;
-        }
-    }
-
     // staging: [voices n][props n] in, [VoiceUpdate n][dirs n][dry][send][hf/lf][FilterUpdate] scratch
     const uint32_t paths = 1u + dd.num_sends;
     CUDA_TRY(d, d->src.wait());
@@ -1614,6 +1523,26 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
             + align16(size_t(cap)*std::max(dd.dry_channels, 1u)*4) + align16(size_t(cap)*std::max(dd.num_sends*dd.wet_channels, 1u)*4)
             + align16(size_t(cap)*(1u + B200MIX_MAX_SENDS)*8) + align16(size_t(cap)*paths*sizeof(FilterUpdate));
         CUDA_TRY(d, d->src.reserve(n, cap, in, in + out + 64, d->stream));
+    }
+
+    if(mayFilter) d->book.set_device_filters();
+    for(uint32_t i = 0;i < n;++i)
+    {
+        const b200mix_source_voice &p = voices[i];
+        const bool act = !(p.flags & B200MIX_VF_STOPPED);
+        // the voice no longer plays a callback buffer
+        if(!d->cbv.empty() && d->cbv[p.voice].slot >= 0)
+        {
+            d->cbv[p.voice].slot = -1;
+            --d->cb_bound;
+        }
+        // the step is not known here: the cost key takes the resampler's widest filter, and is
+        // kept while the voice stays active
+        const BsincTable *t = bsinc_for(d, p.resampler);
+        uint32_t cost = d->book.cost[p.voice];
+        if(bool(d->book.active[p.voice]) != act || (!cost && act)) cost = t ? t->m[0] : (p.resampler >= 2u ? 4u : 2u);
+        d->book.set(p.voice, {act, cost, hrtfMode, p.send_slot,
+            (p.flags & B200MIX_VF_STATIC) ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0});
     }
     UploadArena &U = d->src;
     U.begin();
@@ -1649,23 +1578,10 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
     CUDA_TRY(d, launch_calc_voices(Q, filters, d->stream));
     d->launches += filters ? 2 : 1;
 
-    ApplyParams A{};
-    A.voices = d->d_voices; A.updates = Q.updates;
-    if(hrtfMode)
-    {
-        A.dirs = Q.dirs;
-        A.st_fields = d->d_st_fields; A.st_elevs = d->d_st_elevs; A.st_coeffs = d->d_st_coeffs;
-        A.st_delays = d->d_st_delays; A.st_num_fields = d->st_num_fields; A.st_ir = d->st_ir;
-    }
+    ApplyParams A = apply_params(d, Q.updates);
+    if(hrtfMode) apply_dirs(d, A, Q.dirs);
     else A.dry = Q.dry;
     A.send = Q.send;
-    A.hrtf_tgt = d->d_hrtf_tgt; A.hrtf_old = d->d_hrtf_old;
-    A.dry_cur = d->d_dry_cur; A.dry_tgt = d->d_dry_tgt;
-    A.send_cur = d->d_send_cur; A.send_tgt = d->d_send_tgt;
-    A.ir = dd.ir_size; A.ir_pad = d->ir_pad; A.cd = dd.dry_channels; A.cw = dd.wet_channels;
-    A.num_sends = dd.num_sends;
-    A.filt = d->d_filt; A.filt_paths = paths;
-    A.qhdr = d->d_qhdr;
     k_apply_updates<<<n, 64, 0, d->stream>>>(A);
     ++d->launches;
     if(filters)
@@ -1764,7 +1680,6 @@ static int ensure_filters(b200mix_device *d)
     CUDA_TRY(d, cudaGetLastError());
     ++d->launches;
     d->d_filt = std::move(filt); d->d_dline = std::move(dline); d->d_order2 = std::move(order2);
-    d->h_dfilt.assign(dd.max_voices, 0);
     return B200MIX_OK;
 }
 
@@ -1782,11 +1697,7 @@ int b200mix_voices_filters(b200mix_device *d, uint32_t n, const b200mix_voice_fi
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     if(int rc = ensure_filters(d)) return rc;
     for(uint32_t i = 0;i < n;++i)
-        if(filters[i].path == 0)
-        {
-            const uint8_t act = filters[i].active ? 1 : 0;
-            if(d->h_dfilt[filters[i].voice] != act) { d->h_dfilt[filters[i].voice] = act; d->order2_dirty = true; }
-        }
+        if(filters[i].path == 0) d->book.set_direct_filter(filters[i].voice, filters[i].active != 0);
     UploadArena &U = d->fstage;
     CUDA_TRY(d, U.wait());
     const size_t cap = std::max<size_t>(n, 2u*U.capacity());
@@ -1952,7 +1863,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     // clear MixBuffer (alc/alu.cpp:2417) and the wet buffers (alc/alu.cpp:2196-2198)
     // (the dry mix is left alone while nothing can write or read it: HRTF-only scenes; an
     // HRTF post-process whose RealOut is just L/R overwrites it instead of accumulating)
-    if(d->dry_active || dd.post_process != B200MIX_POST_HRTF)
+    if(d->book.dry_active || dd.post_process != B200MIX_POST_HRTF)
         CUDA_TRY(d, cudaMemsetAsync(d->d_dry, 0, size_t(d->dry_alloc_ch)*kLine*sizeof(float), d->stream));
     d->real_overwrite = dd.post_process == B200MIX_POST_HRTF && dd.real_channels == 2
         && dd.real_left != dd.real_right;
@@ -1961,34 +1872,30 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     if(d->d_wet)
         CUDA_TRY(d, cudaMemsetAsync(d->d_wet, 0, size_t(dd.max_slots)*dd.wet_channels*kLine*sizeof(float), d->stream));
 
-    if(d->order_dirty)
+    VoiceBook &B = d->book;
+    const VoiceBook::Rebuilt re = B.refresh(d->d_filt != nullptr, d->mix_cdr == 0 && d->d_dry_entries,
+        (d->active_slots || force_sends) && d->d_wet && d->d_slot_start);
+    if(re.order)
+        if(int rc = upload(d, d->d_order, B.order)) return rc;
+    if(re.order2)
+        if(int rc = upload(d, d->d_order2, B.order2)) return rc;
+    if(re.dry)
     {
-        d->h_order.clear();
-        for(uint32_t v = 0;v < d->voice_hi;++v) if(d->h_active[v]) d->h_order.push_back(v);
-        std::stable_sort(d->h_order.begin(), d->h_order.end(),
-            [d](uint32_t a, uint32_t b) { return d->h_cost[a] > d->h_cost[b]; });
-        d->num_order = uint32_t(d->h_order.size());
-        if(d->num_order)
-            if(int rc = upload(d, d->d_order, d->h_order)) return rc;
-        d->order_dirty = false;
-        d->order2_dirty = true;
-        d->dry_entries_dirty = true;
+        const uint32_t ss[2] = {0u, uint32_t(B.dry_entries.size())};
+        CUDA_TRY(d, cudaMemcpyAsync(d->d_dry_slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, d->stream));
+        if(int rc = upload(d, d->d_dry_entries, B.dry_entries)) return rc;
     }
-    if(d->d_filt && d->order2_dirty)
+    if(re.sends)
     {
-        d->h_order2.clear();
-        // with the GPU parameter stage the host does not know which direct filters are active:
-        // k_filters and k_mix_deferred then look at every voice's kSiDeferred bit
-        for(uint32_t v : d->h_order) if(d->dev_filters || d->h_dfilt[v]) d->h_order2.push_back(v);
-        d->num_order2 = uint32_t(d->h_order2.size());
-        if(d->num_order2)
-            if(int rc = upload(d, d->d_order2, d->h_order2)) return rc;
-        d->order2_dirty = false;
+        if(int rc = upload(d, d->d_slot_start, B.slot_start)) return rc;
+        if(int rc = upload(d, d->d_entries, B.entries)) return rc;
     }
+    const uint32_t numOrder = uint32_t(B.order.size()), numOrder2 = uint32_t(B.order2.size());
+    const uint32_t numDry = uint32_t(B.dry_entries.size()), numEntries = uint32_t(B.entries.size());
     const bool hrtfDev = dd.ir_size > 0;
-    const uint32_t nv = std::max(d->voice_hi, 1u);
+    const uint32_t nv = std::max(B.voice_hi, 1u);
     const uint32_t maxBlocks = uint32_t(d->num_sms*d->mix_blocks_per_sm);
-    const uint32_t blocks = std::max(1u, std::min(maxBlocks, (d->num_order + kMixGroups - 1)/kMixGroups));
+    const uint32_t blocks = std::max(1u, std::min(maxBlocks, (numOrder + kMixGroups - 1)/kMixGroups));
 
     MixParams P{};
     P.voices = d->d_voices; P.buffers = d->d_buffers;
@@ -2000,7 +1907,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     for(int i = 0;i < 2;++i) P.cubic_tab[i] = d->d_cubic[i];
     P.max_voices = nv; P.frames = frames; P.ir_pad = d->ir_pad;
     P.cd = dd.dry_channels; P.num_sends = dd.num_sends;
-    P.order = d->d_order; P.num_order = d->num_order;
+    P.order = d->d_order; P.num_order = numOrder;
     P.xscratch = d->d_xscratch; P.sendinfo = d->d_sendinfo;
     P.filt = d->d_filt; P.filt_paths = 1u + dd.num_sends;
     P.qhdr = d->d_qhdr; P.queue = d->d_queue;
@@ -2018,23 +1925,23 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     stage_mark(d, 2);
     // ---- voices with an active direct filter: filter the parked lines, then mix them ----
     size_t rows2 = 0;
-    if(d->d_filt && d->num_order2)
+    if(d->d_filt && numOrder2)
     {
         FilterRunParams FP{};
         FP.filt = d->d_filt; FP.filt_paths = 1u + dd.num_sends; FP.sendinfo = d->d_sendinfo;
-        FP.direct_order = d->d_order2; FP.num_direct = d->num_order2;
+        FP.direct_order = d->d_order2; FP.num_direct = numOrder2;
         FP.xscratch = d->d_xscratch; FP.dline = d->d_dline; FP.frames = frames;
-        k_filters<<<(d->num_order2 + 31u)/32u, 32, 0, d->stream>>>(FP);
+        k_filters<<<(numOrder2 + 31u)/32u, 32, 0, d->stream>>>(FP);
         ++d->launches;
         if(d->mix_cdr > 0)
         {
             // The grid is the number of partial rows, so it fixes the order in which the
             // deferred voices' sums are added: it follows the resample kernel's occupancy, as
             // the main pass's does, not this kernel's own.
-            const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (d->num_order2 + kMixGroups - 1)/kMixGroups));
+            const uint32_t blocks2 = std::max(1u, std::min(maxBlocks, (numOrder2 + kMixGroups - 1)/kMixGroups));
             rows2 = blocks2;
             MixParams P2 = P;
-            P2.order = d->d_order2; P2.num_order = d->num_order2;
+            P2.order = d->d_order2; P2.num_order = numOrder2;
             P2.partial = d->d_partial + d->partial_floats;
             P2.results = nullptr;
             k_mix_deferred<kMixGS, kMixGroups, 4><<<blocks2, kMixGS*kMixGroups,
@@ -2049,7 +1956,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     {
         const FirVariant fir = get_fir(dd.ir_size);
         d->fir_rows = std::max(1u, std::min(uint32_t(d->num_sms*d->fir_blocks_per_sm),
-            (d->num_order + kFirGroups - 1)/kFirGroups));
+            (numOrder + kFirGroups - 1)/kFirGroups));
         // straight behind the resample kernel (no direct filters in between), its set-up runs
         // under the resample kernel's last CTAs
         CUDA_TRY(d, launch_ex(d, d->launches == mixDone, fir.fn, dim3(d->fir_rows), dim3(kFirGS*kFirGroups),
@@ -2077,18 +1984,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     // ---- parked dry bus: non-HRTF voices of a variant without register accumulators ----
     if(d->mix_cdr == 0 && d->d_dry_entries)
     {
-        if(d->dry_entries_dirty)
-        {
-            d->h_dry_entries.clear();
-            for(uint32_t v = 0;v < d->voice_hi;++v)
-                if(d->h_active[v] && !d->h_hrtf[v]) d->h_dry_entries.push_back(SendEntry{v, 0u});
-            d->num_dry_entries = uint32_t(d->h_dry_entries.size());
-            const uint32_t ss[2] = {0u, d->num_dry_entries};
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_dry_slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, d->stream));
-            if(int rc = upload(d, d->d_dry_entries, d->h_dry_entries)) return rc;
-            d->dry_entries_dirty = false;
-        }
-        if(d->num_dry_entries)
+        if(numDry)
         {
             SendMixParams DM{};
             DM.slot_start = d->d_dry_slot_start; DM.entries = d->d_dry_entries; DM.sendinfo = d->d_sendinfo;
@@ -2097,14 +1993,14 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
             DM.valid_bit = kSiDry; DM.dline = d->d_dline ? d->d_dline : d->d_xscratch;
             // a CTA's 8 warps share its entries evenly: chunks of 64 entries keep the first
             // (fading) tile's serial work per warp short
-            const uint32_t chunks = std::max(1u, std::min(kDryChunksMax, (d->num_dry_entries + 63u)/64u));
+            const uint32_t chunks = std::max(1u, std::min(kDryChunksMax, (numDry + 63u)/64u));
             DM.chunks = chunks; DM.partial = d->d_dry_partial; DM.geff = d->d_dry_geff; DM.gramp = d->d_dry_gramp;
             // Above 4 dry channels (third-order output) a full update's pan-mix past the gain fades
             // is a dense GEMM over the voices: samples 128..1023 go to the tensor cores
             // (k_panmix_tc), k_send_mix keeps the first tile with the fades
             const bool tc = d->panmix_tc && dd.dry_channels > 4u && dd.dry_channels <= uint32_t(kPmN)
                 && frames == uint32_t(kLine) && chunks > 1u;
-            if(int rc = run_bus_mix(d, DM, d->num_dry_entries, 1u, tc)) return rc;
+            if(int rc = run_bus_mix(d, DM, numDry, 1u, tc)) return rc;
         }
     }
 
@@ -2112,57 +2008,34 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     // ---- aux sends (core/voice.cpp:967-980) ----
     if((d->active_slots || force_sends) && d->d_wet && d->d_slot_start)
     {
-        if(d->sends_dirty)
-        {
-            // CSR of (voice, send) pairs per slot, voices in index order (deterministic sums)
-            d->h_slot_start.assign(dd.max_slots + 1, 0);
-            d->h_entries.clear();
-            for(uint32_t sl = 0;sl < dd.max_slots;++sl)
-            {
-                d->h_slot_start[sl] = uint32_t(d->h_entries.size());
-                for(uint32_t v = 0;v < d->voice_hi;++v)
-                    for(uint32_t s2 = 0;s2 < dd.num_sends;++s2)
-                        if(d->h_send_slot[size_t(v)*B200MIX_MAX_SENDS + s2] == sl)
-                            d->h_entries.push_back(SendEntry{v, s2});
-            }
-            d->h_slot_start[dd.max_slots] = uint32_t(d->h_entries.size());
-            d->num_entries = uint32_t(d->h_entries.size());
-            d->max_slot_entries = 0;
-            for(uint32_t sl = 0;sl < dd.max_slots;++sl)
-                d->max_slot_entries = std::max(d->max_slot_entries, d->h_slot_start[sl+1] - d->h_slot_start[sl]);
-            CUDA_TRY(d, cudaMemcpyAsync(d->d_slot_start, d->h_slot_start.data(),
-                (dd.max_slots + 1)*sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
-            if(int rc = upload(d, d->d_entries, d->h_entries)) return rc;
-            d->sends_dirty = false;
-        }
         SendMixParams SM{};
         SM.slot_start = d->d_slot_start; SM.entries = d->d_entries; SM.sendinfo = d->d_sendinfo;
         SM.xscratch = d->d_xscratch; SM.send_cur = d->d_send_cur; SM.send_tgt = d->d_send_tgt;
         SM.wet = d->d_wet; SM.frames = frames; SM.cw = dd.wet_channels; SM.num_sends = dd.num_sends;
         SM.valid_bit = kSiSend;
-        if(d->d_filt && d->num_entries)
+        if(d->d_filt && numEntries)
         {
-            if(d->d_fscratch.size() < size_t(d->num_entries)*kLine)
+            if(d->d_fscratch.size() < size_t(numEntries)*kLine)
             {
-                CUDA_TRY(d, regrow(d->d_fscratch, size_t(std::max(d->num_entries, 64u))*kLine, d->stream));
+                CUDA_TRY(d, regrow(d->d_fscratch, size_t(std::max(numEntries, 64u))*kLine, d->stream));
                 CUDA_TRY(d, cudaMemsetAsync(d->d_fscratch, 0, d->d_fscratch.bytes(), d->stream));
             }
             SM.filt = d->d_filt; SM.filt_paths = 1u + dd.num_sends; SM.fscratch = d->d_fscratch;
             FilterRunParams FP{};
             FP.filt = d->d_filt; FP.filt_paths = 1u + dd.num_sends; FP.sendinfo = d->d_sendinfo;
-            FP.entries = d->d_entries; FP.num_entries = d->num_entries;
+            FP.entries = d->d_entries; FP.num_entries = numEntries;
             FP.xscratch = d->d_xscratch; FP.fscratch = d->d_fscratch; FP.frames = frames;
-            k_filters<<<(d->num_entries + 31u)/32u, 32, 0, d->stream>>>(FP);
+            k_filters<<<(numEntries + 31u)/32u, 32, 0, d->stream>>>(FP);
             ++d->launches;
         }
         SM.geff = d->d_send_geff; SM.gramp = d->d_send_gramp;
         // a CTA's 8 warps share its entries evenly: chunks of 128 entries per slot
-        const uint32_t chunks = std::max(1u, std::min(16u, (d->max_slot_entries + 127u)/128u));
+        const uint32_t chunks = std::max(1u, std::min(16u, (B.max_slot_entries + 127u)/128u));
         const size_t partialFloats = size_t(chunks)*dd.max_slots*dd.wet_channels*kLine;
         if(chunks > 1u && d->d_send_partial.size() < partialFloats)
             CUDA_TRY(d, regrow(d->d_send_partial, partialFloats, d->stream));
         SM.chunks = chunks; SM.partial = d->d_send_partial;
-        if(int rc = run_bus_mix(d, SM, d->num_entries, dd.max_slots, false)) return rc;
+        if(int rc = run_bus_mix(d, SM, numEntries, dd.max_slots, false)) return rc;
     }
     return B200MIX_OK;
 }
@@ -2298,8 +2171,8 @@ static int render_phase_b(b200mix_device *d, uint32_t frames)
         Q.dry = d->d_dry; Q.real = d->d_real; Q.dec_coef = d->d_dec_coef;
         Q.dec_hfscale = d->d_dec_hfscale; Q.dec_state = d->d_dec_state; Q.temp = d->d_temp;
         Q.frames = frames; Q.cd = dd.dry_channels; Q.dec_ir = d->dec_ir;
-        Q.real_left = dd.real_left; Q.real_right = dd.real_right; Q.dry_active = d->dry_active;
-        if(d->dry_active)
+        Q.real_left = dd.real_left; Q.real_right = dd.real_right; Q.dry_active = d->book.dry_active;
+        if(d->book.dry_active)
         {
             k_post_hrtf_split<<<dd.dry_channels, 32, 0, d->stream>>>(Q);
             ++d->launches;
@@ -2495,7 +2368,7 @@ static int render_collect(b200mix_device *d, uint32_t frames, float *const *real
     b200mix_voice_result *results)
 {
     const b200mix_device_desc &dd = d->desc;
-    const uint32_t nv = std::max(d->voice_hi, 1u);
+    const uint32_t nv = std::max(d->book.voice_hi, 1u);
     const bool contiguous = d->d_real == reinterpret_cast<float*>(d->d_outblock.get());
     if(real_out && results && contiguous)
         CUDA_TRY(d, cudaMemcpyAsync(d->h_outblock, d->d_outblock, d->out_real_bytes + size_t(nv)*sizeof(VoiceResult),

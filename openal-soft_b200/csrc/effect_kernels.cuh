@@ -49,8 +49,6 @@ struct SlotRec {
 };
 
 // ---- send mix --------------------------------------------------------------------------
-struct SendEntry { uint32_t voice, send; };
-
 struct SendMixParams {
     const uint32_t *slot_start;     // [slots+1] CSR over entries
     const SendEntry *entries;

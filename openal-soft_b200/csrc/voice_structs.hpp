@@ -1,6 +1,6 @@
 // voice_structs.hpp — plain records shared by the mixer kernels (mixer_kernels.cuh) and the
 // parameter kernel (param_kernels.cu): what b200mix_voices_update / b200mix_sources_update stage
-// for k_apply_updates and k_apply_filter_updates.
+// for k_apply_updates and k_apply_filter_updates, and the bus mixes' (voice, send) entries.
 #pragma once
 #include <cstdint>
 
@@ -19,5 +19,7 @@ struct alignas(16) VoiceUpdate {   // staged by b200mix_voices_update
 struct FilterUpdate {      // == b200mix_voice_filter
     uint32_t voice, path, active; float lp[5], hp[5];
 };
+
+struct SendEntry { uint32_t voice, send; };   // a voice's send (0 on the dry bus)
 
 } // namespace b200mix

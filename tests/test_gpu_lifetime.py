@@ -4,6 +4,8 @@
   create / configure / render / destroy 20 times; the free device memory must come back.
 - Growth: each upload arena and scratch array grows mid-stream, and the scene still matches the
   CPU oracle within test_gpu_parity's bounds (positions and flags identical).
+- Rejected updates: a voices_update / voices_update_dirs / sources_update call with one bad entry
+  changes neither what the device renders nor which buffers its voices hold.
 - Device guard (two or more GPUs): the output-stage setters allocate on the mixer's GPU whichever
   GPU is current, so a mixer on the last GPU renders what the same scene renders on GPU 0."""
 import ctypes as C
@@ -282,6 +284,110 @@ def test_sources_update_arena_grows_mid_stream():
     assert np.abs(a).max() > 1e-3
     err = a.astype(np.float64) - b
     assert np.sqrt((err ** 2).mean()) <= RMS_TOL and np.abs(err).max() <= MAX_TOL, np.abs(err).max()
+
+
+# ---- rejected updates ----------------------------------------------------------------------
+
+ERR_INVALID = -1                       # B200MIX_ERR_INVALID
+BUF_A, BUF_B, BUF_C = 0, 1, 2
+
+
+def _rejection_device(L, entry, hrtf):
+    """Two convolution slots; voice 0 plays static buffer A into slot 0, voice 1 plays buffer C."""
+    desc = synth.hrtf_desc(4, 64) if entry == "voices_update_dirs" else synth.stereo_desc(4)
+    desc.num_sends, desc.wet_channels, desc.max_slots, desc.max_buffers = 1, 4, 2, 3
+    cd = desc.dry_channels
+    dev = MixDevice(mixlib.product(), desc)
+    if entry == "voices_update_dirs":
+        dev.set_hrtf_decoder(*synth.decoder(np.random.default_rng(7)))
+        assert L.b200mix_hrtf_attach(dev.h, hrtf) == 0
+    else:
+        dev.set_ambi_decoder((np.random.default_rng(8).standard_normal((cd, 2)) * 0.5).astype(np.float32), None, 0.0)
+    for b in (BUF_A, BUF_B, BUF_C):
+        dev.buffer_data(b, abi.FMT_I16, scene.voice_buffer_fast(b))
+    rng = np.random.default_rng(31)
+    for slot in (0, 1):
+        dev.slot_convolution(slot, (rng.standard_normal((4, 300)) * 0.1).astype(np.float32),
+                             np.eye(4, cd, dtype=np.float32) * 0.5)
+    return dev
+
+
+def _apply(L, dev, entry, records, keep):
+    """One update call of the entry point under test; returns its result code."""
+    n, cd = len(records), dev.desc.dry_channels
+    if entry == "sources_update":
+        sv = (SourceVoice * n)(*records)
+        env = _env(keep, cd, 1, 4, 0)
+        return L.b200mix_sources_update(dev.h, n, sv, _props(np.random.default_rng(41), n, 1, True),
+                                        C.byref(_listener(L, np.random.default_rng(42))), C.byref(env))
+    vp = (abi.VoiceParams * n)(*records)
+    send = np.full((n, 1, 4), 0.4, dtype=np.float32)
+    if entry == "voices_update_dirs":
+        dirs = np.tile(np.array([[0.2, 0.8, 1.5, 0.0]], dtype=np.float32), (n, 1))
+        return L.b200mix_voices_update_dirs(dev.h, n, vp, dirs.ctypes.data, None, send.ctypes.data)
+    dry = (np.random.default_rng(43).standard_normal((n, cd)) * 0.3).astype(np.float32)
+    return dev.m.voices_update(dev.h, n, vp, None, dry.ctypes.data, send.ctypes.data)
+
+
+def _record(entry, voice, buffer, slot):
+    r = SourceVoice() if entry == "sources_update" else abi.VoiceParams()
+    r.voice, r.buffer, r.resampler = voice, buffer, abi.RS_SPLINE
+    r.flags = abi.VF_PLAYING | abi.VF_STATIC | abi.VF_LOOPING | abi.VF_RESET
+    if entry == "voices_update_dirs":
+        r.flags |= abi.VF_HRTF
+    r.loop_start, r.loop_end = 0, scene.BUFFER_FRAMES
+    for s in range(abi.MAX_SENDS):
+        r.send_slot[s] = slot if s == 0 else abi.NO_SLOT
+    if entry == "sources_update":
+        r.buffer_rate = 48000
+    else:
+        r.step, r.hrtf_gain = 0x11000, 0.5
+    return r
+
+
+@pytest.mark.parametrize("entry,reject", [
+    ("voices_update", "empty_loop"), ("voices_update", "step"), ("voices_update", "hrtf_delay"),
+    ("voices_update_dirs", "empty_loop"), ("voices_update_dirs", "step"), ("sources_update", "empty_loop")])
+def test_rejected_update_changes_nothing(entry, reject):
+    """A call whose entry 0 moves voice 0 from buffer A / slot 0 to buffer B / slot 1 and whose entry 1
+    is rejected returns B200MIX_ERR_INVALID and changes nothing: four updates render RealOut bit for
+    bit as a twin that never saw the call, and buffer A is still held by its voice while B is not."""
+    if entry == "voices_update_dirs" and not os.path.exists(MHR):
+        pytest.skip("HRTF data set not staged (run build())")
+    L = _L()
+    L.b200mix_buffer_free.argtypes = [C.c_void_p, C.c_uint32]
+    data = open(MHR, "rb").read() if entry == "voices_update_dirs" else None
+    hrtf = C.c_void_p()
+    if data:
+        assert L.b200mix_hrtf_load(data, len(data), C.byref(hrtf)) == 0
+    keep, outs, devs = [], [], []
+    try:
+        devs += [_rejection_device(L, entry, hrtf) for _ in range(2)]
+        for dev in devs:
+            rc = _apply(L, dev, entry, [_record(entry, 0, BUF_A, 0), _record(entry, 1, BUF_C, abi.NO_SLOT)], keep)
+            assert rc == 0, L.b200mix_last_error(dev.h)
+            outs.append([dev.render()])
+        bad = _record(entry, 1, BUF_C, abi.NO_SLOT)
+        if reject == "empty_loop":
+            bad.loop_end = bad.loop_start
+        elif reject == "step":
+            bad.step = (10 << 16) + 1
+        else:
+            bad.hrtf_delay[0] = abi.HRTF_HISTORY
+        moved = _record(entry, 0, BUF_B, 1)
+        assert _apply(L, devs[0], entry, [moved, bad], keep) == ERR_INVALID
+        for dev, out in zip(devs, outs):
+            out += [dev.render() for _ in range(4)]
+        assert np.abs(outs[1][-1]).max() > 1e-4
+        for a, b in zip(*outs):
+            assert a.tobytes() == b.tobytes()
+        assert L.b200mix_buffer_free(devs[0].h, BUF_A) == ERR_INVALID
+        assert L.b200mix_buffer_free(devs[0].h, BUF_B) == 0
+    finally:
+        for dev in devs:
+            dev.close()
+        if data:
+            L.b200mix_hrtf_free(hrtf)
 
 
 # ---- device guard --------------------------------------------------------------------------
