@@ -27,27 +27,6 @@ constexpr int kConvFft = 256;       // ConvolveUpdateSize
 constexpr int kConvMaxBlocks = 9;   // blocks that can complete in one 1024-frame update
 constexpr int kConvMaxChunks = 48;  // segment-range chunks of k_conv_mac (gridDim.z), partials in yspec
 
-struct SlotRec {
-    uint32_t type, channels, frames, segs;     // segs = mNumConvolveSegs
-    uint32_t cur, fifo, nb_last, f_last;       // ring position, FIFO fill; last update's record
-    uint32_t cur_last;
-    uint32_t rv_cur, rv_mask;                  // reverb: current pipeline object; objects to run now
-    uint32_t stage;                            // processing stage: every slot runs before its target
-    float *H;         // [channels][segs][256]  filter spectra (pre-scaled by 1/256)
-    float *X;         // [segs+kConvMaxBlocks][256] input spectra ring (our own ring: long enough that
-                      //                        a whole update's blocks never overwrite live history)
-    float *head;      // [channels][128]        first 128 IR taps
-    float *inbuf;     // [256]                  mInput
-    float *ov;        // [channels][256]        mOutput
-    float *yspec;     // [channels][kConvMaxChunks][kConvMaxBlocks][256] partial sums per segment chunk
-    float *lines;     // [channels][1024]       this update's output lines
-    float *gains;     // [2][channels][32]      ping-pong Current gains
-    float *gtgt;      // [channels][32]         Target gains
-    uint32_t gsel, target;                     // target: slot whose Wet takes the output, or 0xffffffff (Dry)
-    uint32_t fade_len;                         // MixSamples Counter of the output mix: 0 = samplesToDo, else min(n, fade_len)
-    uint32_t pad_;
-};
-
 // ---- send mix --------------------------------------------------------------------------
 struct SendMixParams {
     const uint32_t *slot_start;     // [slots+1] CSR over entries
@@ -513,7 +492,7 @@ __device__ __forceinline__ void fft256_inplace(float2 *data, const float2 *__res
 }
 
 struct ConvParams {
-    SlotRec *slots; const float *wet; const float2 *twiddle;
+    const SlotRec *slots; const float *wet; const float2 *twiddle;
     uint32_t frames, cw, num_slots, stage;
     uint32_t chunks;                  // gridDim.z of k_conv_mac
 };
@@ -528,10 +507,11 @@ __global__ void __launch_bounds__(128) k_conv_input(const ConvParams Q)
     __shared__ float stream[kConvFft + kLine + 8];
     __shared__ float2 fbuf[kConvFft];
     __shared__ float hsm[kConvBlock];
-    SlotRec &S = Q.slots[blockIdx.x];
+    const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 1u || S.stage != Q.stage) return;
+    ConvRing &G = *S.ring;
     const int t = threadIdx.x;
-    const uint32_t n = Q.frames, f = S.fifo, cur = S.cur, ring = S.segs + kConvMaxBlocks;
+    const uint32_t n = Q.frames, f = G.fifo, cur = G.cur, ring = S.segs + kConvMaxBlocks;
     const uint32_t nb = (f + n) / kConvBlock;
     const float *in = Q.wet + size_t(blockIdx.x)*Q.cw*kLine;          // wet channel 0
     // stream = [previous block | partial block (f) | new samples (n)]
@@ -585,9 +565,9 @@ __global__ void __launch_bounds__(128) k_conv_input(const ConvParams Q)
     S.inbuf[kConvBlock + t] = keep1;
     if(t == 0)
     {
-        S.nb_last = nb; S.f_last = f; S.cur_last = cur;
-        S.fifo = fNew;
-        S.cur = (cur + ring - nb) % ring;
+        G.nb_last = nb; G.f_last = f; G.cur_last = cur;
+        G.fifo = fNew;
+        G.cur = (cur + ring - nb) % ring;
     }
 }
 
@@ -616,10 +596,11 @@ __global__ void __launch_bounds__(128) k_conv_mac(const ConvParams Q)
     ConvMacSmem &M = *reinterpret_cast<ConvMacSmem*>(conv_smem_raw);
     const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 1u || S.stage != Q.stage || blockIdx.y >= S.channels) return;
-    const uint32_t nb = S.nb_last;
+    const ConvRing &G = *S.ring;
+    const uint32_t nb = G.nb_last;
     if(nb == 0) return;
     const int t = threadIdx.x;
-    const uint32_t segs = S.segs, cur0 = S.cur_last, ring = segs + kConvMaxBlocks;
+    const uint32_t segs = S.segs, cur0 = G.cur_last, ring = segs + kConvMaxBlocks;
     const uint32_t clen = conv_chunk_len(segs, gridDim.z);
     const uint32_t s0 = blockIdx.z*clen;
     if(s0 >= segs) return;                                   // empty chunk (short IR)
@@ -727,8 +708,8 @@ __global__ void __launch_bounds__(128) k_conv_ifft(const ConvParams Q)
 {
     __shared__ float2 fbuf[kConvFft];
     __shared__ float2 ysp[kConvBlock];
-    SlotRec &S = Q.slots[blockIdx.x];
-    if(S.type != 1u || S.stage != Q.stage || blockIdx.y >= S.channels || blockIdx.z >= S.nb_last) return;
+    const SlotRec &S = Q.slots[blockIdx.x];
+    if(S.type != 1u || S.stage != Q.stage || blockIdx.y >= S.channels || blockIdx.z >= S.ring->nb_last) return;
     const int t = threadIdx.x;
     const uint32_t c = blockIdx.y, b = blockIdx.z;
     const uint32_t clen = conv_chunk_len(S.segs, Q.chunks);
@@ -763,10 +744,10 @@ __global__ void __launch_bounds__(128) k_conv_ifft(const ConvParams Q)
 // (convolution.cpp:699-706) into the slot's output lines.
 __global__ void __launch_bounds__(128) k_conv_output(const ConvParams Q)
 {
-    SlotRec &S = Q.slots[blockIdx.x];
+    const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 1u || S.stage != Q.stage || blockIdx.y >= S.channels) return;
     const int t = threadIdx.x;
-    const uint32_t c = blockIdx.y, n = Q.frames, nb = S.nb_last, f = S.f_last;
+    const uint32_t c = blockIdx.y, n = Q.frames, nb = S.ring->nb_last, f = S.ring->f_last;
     float *ov = S.ov + size_t(c)*kConvFft;
     float *line = S.lines + size_t(c)*kLine;
     float first = ov[t], tail = ov[kConvBlock + t];
@@ -795,7 +776,7 @@ __global__ void __launch_bounds__(128) k_conv_output(const ConvParams Q)
 
 // Dry[o][i] += sum over slots/lines of line[i]*gain(i): MixSamples(Counter = samplesToDo)
 // (ConvolutionState::NormalMix, convolution.cpp:298-304), slots and lines in index order.
-struct SlotMixParams { SlotRec *slots; float *dry; uint32_t frames, cd, num_slots, stage; float *wet; uint32_t cw; };
+struct SlotMixParams { const SlotRec *slots; float *dry; uint32_t frames, cd, num_slots, stage; float *wet; uint32_t cw; };
 
 __global__ void __launch_bounds__(128) k_slot_output_mix(const SlotMixParams Q)
 {
@@ -842,7 +823,7 @@ __global__ void __launch_bounds__(128) k_slot_output_mix(const SlotMixParams Q)
             if(c >= s_ch[sl]) continue;
             const SlotRec &S = Q.slots[sb + sl];
             const uint32_t li = (c + s_first[sl]) & (kMaxLines - 1u);
-            s_cg[sl][c] = S.gains[size_t(S.gsel)*S.channels*32u + li*32u + o];
+            s_cg[sl][c] = S.gains[li*32u + o];
             s_tg[sl][c] = S.gtgt[li*32u + o];
         }
         __syncthreads();
@@ -898,8 +879,9 @@ __global__ void __launch_bounds__(128) k_slot_output_mix(const SlotMixParams Q)
 
 // Slots with a target slot (EffectSlotBase::Target): their output lines are mixed into the
 // target's Wet buffer before the target's stage runs.  grid (tile of 128 samples, target slot);
-// the sources of one target are added in slot order (deterministic).
-__global__ void __launch_bounds__(128) k_slot_target_mix(const SlotMixParams Q)
+// the sources of one target are added in slot order (deterministic).  Full occupancy (16 CTAs per SM)
+// fits in 32 registers.
+__global__ void __launch_bounds__(128, 16) k_slot_target_mix(const SlotMixParams Q)
 {
     const uint32_t t = blockIdx.y;
     const uint32_t i = blockIdx.x*128u + threadIdx.x;
@@ -914,7 +896,7 @@ __global__ void __launch_bounds__(128) k_slot_target_mix(const SlotMixParams Q)
         if(S.type == 2u) { first = S.rv_cur*8u; ch = (S.rv_mask == 3u) ? 16u : 8u; }
         const uint32_t L = S.fade_len ? min(S.fade_len, n) : n;
         const float dl = (L == n) ? delta : 1.0f/float(L);
-        const float *gcur = S.gains + size_t(S.gsel)*S.channels*32u;
+        const float *gcur = S.gains;
         for(uint32_t o = 0;o < Q.cw;++o)
         {
             float acc = Q.wet[(size_t(t)*Q.cw + o)*kLine + i];
@@ -936,14 +918,13 @@ __global__ void __launch_bounds__(128) k_slot_target_mix(const SlotMixParams Q)
 __global__ void k_slot_gains_commit(const SlotMixParams Q)
 {
     const uint32_t s = blockIdx.x;
-    SlotRec &S = Q.slots[s];
+    const SlotRec &S = Q.slots[s];
     if(S.type == 0u) return;
-    float *gcur = S.gains + size_t(S.gsel)*S.channels*32u;
     for(uint32_t k = threadIdx.x;k < S.channels*32u;k += blockDim.x)
     {
         // a reverb pipeline object that did not run this update keeps its Current gains
         if(S.type == 2u && !((S.rv_mask >> (k >> 8)) & 1u)) continue;
-        gcur[k] = S.gtgt[k];
+        S.gains[k] = S.gtgt[k];
     }
 }
 
@@ -979,7 +960,7 @@ struct ReverbDev {
     float *main_d, *late_in, *early_ap, *early_d, *late_ap, *late_d;
 };
 
-struct ReverbParamsK { SlotRec *slots; const float *wet; const float *cubic; uint32_t frames, cw, stage, seq; };
+struct ReverbParamsK { const SlotRec *slots; const float *wet; const float *cubic; uint32_t frames, cw, stage, seq; };
 
 __device__ __forceinline__ void scatter4(const float in[4], float x, float y, float out[4])
 {
@@ -1028,7 +1009,7 @@ __global__ void __launch_bounds__(128) k_reverb_process(const ReverbParamsK Q)
     constexpr uint32_t MAXUPD = 256;
     __shared__ float temp[NL][MAXUPD];
     __shared__ uint32_t moddel[MAXUPD];
-    SlotRec &S = Q.slots[blockIdx.x];
+    const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 2u || S.stage != Q.stage || !((S.rv_mask >> blockIdx.y) & 1u)) return;
     // blockIdx.y = pipeline object (ReverbState::mPipelines[2]); both share the main delay line,
     // each early CTA writes this update's input into it itself (identical values) before reading it.
@@ -1390,7 +1371,7 @@ __global__ void __launch_bounds__(128) k_reverb_process(const ReverbParamsK Q)
 // After both halves of every pipeline: the write offset moves on (ReverbState::mOffset, reverb.cpp:1880).
 __global__ void k_reverb_commit(const ReverbParamsK Q)
 {
-    SlotRec &S = Q.slots[blockIdx.x];
+    const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 2u || S.stage != Q.stage || !((S.rv_mask >> threadIdx.x) & 1u)) return;
     reinterpret_cast<ReverbDev*>(S.H)[threadIdx.x].offset += Q.frames;
 }
@@ -1404,7 +1385,7 @@ __global__ void k_reverb_commit(const ReverbParamsK Q)
 __global__ void __launch_bounds__(256) k_reverb_upmix(const ReverbParamsK Q)
 {
     extern __shared__ float rows[];                 // [8][1024]
-    SlotRec &S = Q.slots[blockIdx.x];
+    const SlotRec &S = Q.slots[blockIdx.x];
     if(S.type != 2u || S.stage != Q.stage || !((S.rv_mask >> blockIdx.y) & 1u)) return;
     ReverbDev &R = reinterpret_cast<ReverbDev*>(S.H)[blockIdx.y];
     if(!R.upmix) return;

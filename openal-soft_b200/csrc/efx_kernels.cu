@@ -141,13 +141,13 @@ __device__ __forceinline__ void hilbert1024_warp(double2 *x, uint32_t lane)
 __global__ void __launch_bounds__(128) k_efx_process(const EfxRunParams Q)
 {
     extern __shared__ float sm[];
-    const EfxSlotView V = Q.slots[blockIdx.x];
-    if(!V.dev || V.stage != Q.stage) return;
-    EfxDev &E = *V.dev;
+    const SlotRec &S = Q.slots[blockIdx.x];
+    if(S.type < B200MIX_EFFECT_ECHO || S.stage != Q.stage) return;
+    EfxDev &E = *reinterpret_cast<EfxDev*>(S.H);
     const EfxParams &P = E.p;
     const uint32_t t = threadIdx.x, n = Q.frames;
     const float *wet = Q.wet + size_t(blockIdx.x)*Q.cw*kLine;
-    float *lines = V.lines;
+    float *lines = S.lines;
     const uint32_t nin = min(P.in_channels, Q.cw);
     float *sIn = sm;                                   // [kEfxMaxLines][1024]
     float *sWork = sm + kEfxMaxLines*kLine;            // [.. ][1024]
@@ -623,14 +623,14 @@ __global__ void __launch_bounds__(128) k_efx_process(const EfxRunParams Q)
 __global__ void __launch_bounds__(128) k_efx_pshift(const EfxRunParams Q)
 {
     extern __shared__ float sm[];
-    const EfxSlotView V = Q.slots[blockIdx.x];
-    if(!V.dev || V.stage != Q.stage) return;
-    EfxDev &E = *V.dev;
+    const SlotRec &S = Q.slots[blockIdx.x];
+    if(S.type < B200MIX_EFFECT_ECHO || S.stage != Q.stage) return;
+    EfxDev &E = *reinterpret_cast<EfxDev*>(S.H);
     const EfxParams &P = E.p;
     if(P.type != B200MIX_EFFECT_PSHIFTER) return;
     const uint32_t t = threadIdx.x, n = Q.frames;
     const float *wet = Q.wet + size_t(blockIdx.x)*Q.cw*kLine;
-    float *lines = V.lines;
+    float *lines = S.lines;
     const uint32_t nin = min(P.in_channels, Q.cw);
     float *sIn = sm;
     float *sWork = sm + kEfxMaxLines*kLine;

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include "efx_math.hpp"
+#include "voice_structs.hpp"
 
 namespace b200mix {
 
@@ -31,8 +32,8 @@ struct EfxDev {
     uint32_t ps_count, ps_pos;
 };
 
-struct EfxSlotView { EfxDev *dev; float *lines; uint32_t stage, pad; };   // dev == null: not an EFX slot
-struct EfxRunParams { const EfxSlotView *slots; const float *wet; uint32_t frames, cw, stage; const float *cubic; /* gCubicTable [513] */ };
+// k_efx_process / k_efx_pshift run the slots of type >= B200MIX_EFFECT_ECHO: their EfxDev is SlotRec::H
+struct EfxRunParams { const SlotRec *slots; const float *wet; uint32_t frames, cw, stage; const float *cubic; /* gCubicTable [513] */ };
 
 cudaError_t efx_kernels_init();            // per CUDA device: dynamic shared memory opt-in
 cudaError_t launch_efx_process(const EfxRunParams &Q, uint32_t num_slots, cudaStream_t stream);

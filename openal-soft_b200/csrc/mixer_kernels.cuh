@@ -976,18 +976,18 @@ __device__ __forceinline__ void mix_dry(float (&accD)[CDR][kLine/GS], const floa
         for(int r = 0;r < SPT;++r)
         {
             const uint32_t i = t + r*GS;
-            float gsel = 0.0f;
+            float gi = 0.0f;
             if(i < n)
-                gsel = (fade && i < fadeLen) ? (cg + step*float(i)) : (i >= start ? flat : 0.0f);
+                gi = (fade && i < fadeLen) ? (cg + step*float(i)) : (i >= start ? flat : 0.0f);
             const float x = xs[i < n ? i : 0];
-            // one fused multiply-add, written out: left to the compiler, whether x*gsel is
+            // one fused multiply-add, written out: left to the compiler, whether x*gi is
             // contracted into the sum depends on the kernel this is inlined into, and both
             // kernels that call this must round the same way
             if(c < uint32_t(CDR))
             {
                 #pragma unroll
                 for(int cc = 0;cc < CDR;++cc)
-                    if(cc == int(c)) accD[cc][r] = __fmaf_rn(x, gsel, accD[cc][r]);
+                    if(cc == int(c)) accD[cc][r] = __fmaf_rn(x, gi, accD[cc][r]);
             }
         }
         if(t == 0)
