@@ -103,11 +103,12 @@ B200MIX_API uint32_t b200mix_version(void);
 /* DirectHrtfState (core/hrtf.h:84-110): per dry channel the pre-summed
  * virtual-speaker HRIR, the HF scale and the band-splitter coefficient.
  * ir_size is DirectHrtfState::mIrSize (may exceed the per-voice ir_size, <=128);
- * coeffs is [channels][ir_size][2]. */
+ * coeffs is [channels][ir_size][2].  Refused between b200mix_render_begin and _render_end. */
 B200MIX_API int b200mix_set_hrtf_decoder(b200mix_device *dev, uint32_t channels,
     uint32_t ir_size, const float *coeffs, const float *hf_scale, const float *splitter_coeff);
 /* BFormatDec (core/bformatdec.h): gains_hf/gains_lf are [in_channels][real_channels];
- * gains_lf==NULL selects the single-band decoder; xover_coeff is the splitter's mCoeff. */
+ * gains_lf==NULL selects the single-band decoder; xover_coeff is the splitter's mCoeff.
+ * Refused between b200mix_render_begin and _render_end. */
 B200MIX_API int b200mix_set_ambi_decoder(b200mix_device *dev, uint32_t in_channels,
     const float *gains_hf, const float *gains_lf, float xover_coeff);
 

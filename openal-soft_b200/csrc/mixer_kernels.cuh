@@ -2106,7 +2106,7 @@ constexpr MatrixEncSpec kTsmeEncSpec{0u, 3u, 1u, 2u, 0.288397341271f, 0.16656544
     0.444008050325f, -0.256439256487f, 0.333238912931f};
 
 struct PostUhjParams {
-    const float *dry; float *real; float *state; float *scratch;   // scratch [5][1025]
+    const float *dry; float *real; float *state; float *scratch;   // scratch: not read (null)
     uint32_t frames, real_left, real_right;
     MatrixEncSpec enc;
 };
@@ -2763,7 +2763,9 @@ struct OutputParams {
     float dither_depth;
 };
 
-__device__ __forceinline__ uint32_t lcg_skip(uint32_t x, uint32_t k)
+// Also advances the host's seed past an update, whose step count needs 64 bits.
+template<typename Count>
+__host__ __device__ __forceinline__ uint32_t lcg_skip(uint32_t x, Count k)
 {
     // k steps of x -> x*96314165 + 907633515 (dither_rng, alc/alu.cpp:444-448)
     uint32_t a = 96314165u, c = 907633515u;      // one step

@@ -5,7 +5,8 @@
 - Growth: each upload arena and scratch array grows mid-stream, and the scene still matches the
   CPU oracle within test_gpu_parity's bounds (positions and flags identical).
 - Rejected updates: a voices_update / voices_update_dirs / sources_update call with one bad entry
-  changes neither what the device renders nor which buffers its voices hold.
+  changes neither what the device renders nor which buffers its voices hold; an output-stage setter
+  refused for a bad argument or between render_begin and render_end changes nothing either.
 - Device guard (two or more GPUs): the output-stage setters allocate on the mixer's GPU whichever
   GPU is current, so a mixer on the last GPU renders what the same scene renders on GPU 0."""
 import ctypes as C
@@ -388,6 +389,111 @@ def test_rejected_update_changes_nothing(entry, reject):
             dev.close()
         if data:
             L.b200mix_hrtf_free(hrtf)
+
+
+def _output_device(kind):
+    """ambi: 3 RealOut channels, a dual-band decoder, the front stabilizer, a limiter and distance
+    compensation; uhj: the FIR-256 encoder and a limiter; hrtf: its decoder.  64 voices play, a third of
+    them through the dry mix on the HRTF device."""
+    rng = np.random.default_rng(5)
+    if kind == "hrtf":
+        dev = MixDevice(mixlib.product(), synth.hrtf_desc(64, 64))
+        dev.set_hrtf_decoder(*synth.decoder(np.random.default_rng(7)))
+        params, coeffs, dry = synth.voice_set(rng, 64, 64)
+        for k in range(1, 64, 3):
+            params[k].flags &= ~abi.VF_HRTF
+    else:
+        desc = synth.stereo_desc(64, dry_channels=4 if kind == "ambi" else 3)
+        if kind == "ambi":
+            desc.real_channels = 3
+        else:
+            desc.post_process = abi.POST_UHJ
+        dev = MixDevice(mixlib.product(), desc)
+        if kind == "ambi":
+            gains = (rng.standard_normal((2, 4, 3)) * 0.5).astype(np.float32)
+            dev.set_ambi_decoder(gains[0], gains[1], -0.9123257)
+            dev.set_front_stabilizer(2, -0.9123257)
+            dev.set_distance_comp([3, 5, 1], [1.0, 0.9, 0.8])
+        else:
+            dev.set_uhj_encoder(256)
+        dev.set_limiter(abi.device_limiter(-6.0))
+        params, coeffs, dry = synth.voice_set(rng, 64, 0, hrtf=False, dry_channels=desc.dry_channels,
+                                              resampler=abi.RS_SPLINE)
+        coeffs = None
+    for i in range(64):
+        dev.buffer_data(i, abi.FMT_I16, scene.voice_buffer_fast(i))
+    dev.voices_update(params, coeffs, dry, None)
+    return dev
+
+
+def _output_call(dev, call):
+    """One output-stage call through the C ABI; returns its result code."""
+    m, h = dev.m, dev.h
+    rng = np.random.default_rng(11)
+    lim = abi.device_limiter(-3.0)
+    if call == "limiter_struct_size":
+        lim.struct_size += 4
+    gains = (rng.standard_normal((4, 3)) * 0.5).astype(np.float32)
+    cd = 3 if call == "hrtf_decoder_channels" else 4
+    dec = synth.decoder(rng, channels=cd)
+    delays = np.array([3, 5, 1024 if call == "distance_comp_delay" else 1, 2], dtype=np.uint32)
+    dc_gains = np.array([1.0, 0.9, 0.8, 0.7], dtype=np.float32)
+    calls = {
+        "distance_comp_delay": lambda: m.set_distance_comp(h, 3, delays.ctypes.data, dc_gains.ctypes.data),
+        "distance_comp_channels": lambda: m.set_distance_comp(h, 4, delays.ctypes.data, dc_gains.ctypes.data),
+        "limiter_struct_size": lambda: m.set_limiter(h, C.byref(lim), None),
+        "bs2b_level_7": lambda: m.set_bs2b(h, 7),
+        "stabilizer_on_left": lambda: m.set_front_stabilizer(h, dev.desc.real_left, -0.9),
+        "uhj_length_128": lambda: m.set_uhj_encoder(h, 128, None),
+        "ambi_decoder_channels": lambda: m.set_ambi_decoder(h, 3, gains[:3].ctypes.data, None, 0.0),
+        "hrtf_decoder_channels": lambda: m.set_hrtf_decoder(h, cd, dec[0].shape[1], dec[0].ctypes.data,
+                                                            dec[1].ctypes.data, dec[2].ctypes.data),
+        # accepted outside a render
+        "hrtf_decoder": lambda: m.set_hrtf_decoder(h, cd, dec[0].shape[1], dec[0].ctypes.data, dec[1].ctypes.data,
+                                                   dec[2].ctypes.data),
+        "ambi_decoder": lambda: m.set_ambi_decoder(h, 4, gains.ctypes.data, gains.ctypes.data, -0.8),
+        "uhj_encoder": lambda: m.set_uhj_encoder(h, 512, None),
+        "front_stabilizer": lambda: m.set_front_stabilizer(h, 2, -0.8),
+        "bs2b": lambda: m.set_bs2b(h, 3),
+        "distance_comp": lambda: m.set_distance_comp(h, 2, delays.ctypes.data, dc_gains.ctypes.data),
+        "limiter": lambda: m.set_limiter(h, C.byref(lim), None),
+    }
+    return calls[call]()
+
+
+@pytest.mark.parametrize("kind,call,mid_render", [
+    ("ambi", "distance_comp_delay", False), ("ambi", "distance_comp_channels", False),
+    ("ambi", "limiter_struct_size", False), ("ambi", "bs2b_level_7", False), ("ambi", "stabilizer_on_left", False),
+    ("uhj", "uhj_length_128", False), ("ambi", "ambi_decoder_channels", False),
+    ("hrtf", "hrtf_decoder_channels", False),
+    ("hrtf", "hrtf_decoder", True), ("ambi", "ambi_decoder", True), ("uhj", "uhj_encoder", True),
+    ("ambi", "front_stabilizer", True), ("ambi", "bs2b", True), ("ambi", "distance_comp", True),
+    ("uhj", "limiter", True)])
+def test_rejected_output_stage_call_changes_nothing(kind, call, mid_render):
+    """An output-stage setter refused with B200MIX_ERR_INVALID, for a bad argument or between render_begin
+    and render_end (with arguments it accepts outside a render), changes nothing: RealOut of the update it
+    interrupts and of four more is bit for bit a twin's that never saw the call."""
+    devs = [_output_device(kind) for _ in range(2)]
+    try:
+        outs = [[dev.render()] for dev in devs]
+        if mid_render:
+            for dev in devs:
+                dev.render_begin()
+        assert _output_call(devs[0], call) == ERR_INVALID
+        if mid_render:
+            assert "render_begin is pending" in devs[0].last_error()
+            for dev, out in zip(devs, outs):
+                out.append(dev.render_end())
+        for dev, out in zip(devs, outs):
+            out += [dev.render() for _ in range(4)]
+        assert np.abs(outs[1][-1]).max() > 1e-4
+        for a, b in zip(*outs):
+            assert a.tobytes() == b.tobytes()
+        if mid_render:
+            assert _output_call(devs[0], call) == 0, devs[0].last_error()
+    finally:
+        for dev in devs:
+            dev.close()
 
 
 # ---- device guard --------------------------------------------------------------------------
