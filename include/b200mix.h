@@ -408,7 +408,12 @@ enum {
     B200MIX_VF_RESET     = 1u<<5, /* fresh voice (Voice::prepare): zero histories, take position,
                                      clear IsFading */
     B200MIX_VF_FADING    = 1u<<6, /* with RESET: start with IsFading set (al/source.cpp:775,2714) */
-    B200MIX_VF_STOPPED   = 1u<<7  /* Voice::Stopped: remove from the active set */
+    B200MIX_VF_STOPPED   = 1u<<7, /* Voice::Stopped: remove from the active set */
+    B200MIX_VF_DIRECT    = 1u<<8  /* direct channels (AL_DIRECT_CHANNELS_SOFT): the direct path is
+                                     RealOut (mDirect.Buffer = RealOut.Buffer).  Only
+                                     b200mix_voices_update_direct takes it (and requires it); the
+                                     other update calls ignore the bit and mix the voice into Dry
+                                     or through its HRIR */
 };
 /* Multi-channel sources: the reference mixes every buffer channel as its own mixing channel
  * with its own panning/HRIR (Voice::mChans[c], core/voice.h:236-257; LoadSamples' srcChannel,
@@ -880,6 +885,26 @@ B200MIX_API int b200mix_get_voice_targets(b200mix_device *dev, uint32_t voice, u
 B200MIX_API int b200mix_voices_update_dirs(b200mix_device *dev, uint32_t n,
     const b200mix_voice_params *params, const float *dirs, const float *dry_gains,
     const float *send_gains);
+/* Direct-channel voices (CalcDirectPanning, alc/alu.cpp:1142-1195): every entry carries
+ * B200MIX_VF_DIRECT and not B200MIX_VF_HRTF, and its direct path mixes into RealOut ahead of the
+ * post-process:
+ *   real_gains [n][real_channels]           mDryParams.Gains.Target by RealOut channel (may be NULL)
+ *   send_gains [n][num_sends][wet_channels] as in b200mix_voices_update (may be NULL)
+ * A NULL side array leaves those targets unchanged.  The direct filter (path 0 of
+ * b200mix_voices_filters) and the sends work as for any voice.  A voice keeps one set of Current
+ * gains whichever mix it feeds, as the reference's voice does: switched between this call and
+ * b200mix_voices_update(_dirs) while it plays, it fades from the gains it last had at each
+ * channel index.  A later b200mix_voices_update(_dirs) of the voice returns it to the Dry / HRTF
+ * path.
+ * B200MIX_ERR_UNSUPPORTED, with nothing applied, where the reference never mixes direct
+ * channels (RealOut.RemixMap is empty or RealOut is the Dry mix): B200MIX_POST_NONE, UHJ and
+ * TSME devices; and, not supported here: sharded device sets and devices with a front
+ * stabilizer (while a direct voice is active, b200mix_set_front_stabilizer and joining a set of
+ * more than one device through b200mix_shard_init / b200mix_shard_nccl are refused the same way).  The
+ * BS2B and HRTF post-processes leave the direct signal unfiltered, as the reference's do.
+ * b200mix_sources_update has no direct mode. */
+B200MIX_API int b200mix_voices_update_direct(b200mix_device *dev, uint32_t n,
+    const b200mix_voice_params *params, const float *real_gains, const float *send_gains);
 
 /* ---- introspection (tests, profiling) ------------------------------------ */
 /* Copies the Dry mix of the last update: [dry_channels][1024]. */

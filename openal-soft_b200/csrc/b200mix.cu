@@ -104,6 +104,11 @@ struct b200mix_device {
     DevArray<float> d_send_geff;             // [max_voices*num_sends][cw]
     DevArray<float4> d_dry_gramp, d_send_gramp;
     DevArray<float> d_send_partial;          // [send_chunks][max_slots][cw][1024]
+    // RealOut bus of the direct-channel voices (allocated by the first b200mix_voices_update_direct)
+    DevArray<SendEntry> d_real_entries; DevArray<uint32_t> d_real_slot_start;   // book.real_entries
+    DevArray<float> d_real_cur, d_real_tgt, d_real_geff;   // [max_voices][real_channels]
+    DevArray<float4> d_real_gramp;
+    bool real_mixed{false};                  // the last update mixed the RealOut bus
     bool profile{false};
     Event ev_mix0, ev_mix1;
     bool ev_valid{false};
@@ -245,6 +250,28 @@ int ensure_dry_park(b200mix_device *d)
     return B200MIX_OK;
 }
 
+// Storage of the RealOut bus (the first direct-channel voice): the parked lines, the voices'
+// RealOut gains and the bus' entries.
+int ensure_real_bus(b200mix_device *d)
+{
+    const b200mix_device_desc &dd = d->desc;
+    if(d->d_real_entries) return B200MIX_OK;
+    if(int rc = ensure_park_lines(d)) return rc;
+    const size_t gains = size_t(dd.max_voices)*dd.real_channels;
+    DevArray<SendEntry> entries; DevArray<uint32_t> slotStart;
+    DevArray<float> cur, tgt, geff; DevArray<float4> gramp;
+    CUDA_TRY(d, entries.alloc(dd.max_voices, d->stream));
+    CUDA_TRY(d, slotStart.alloc(2, d->stream));
+    CUDA_TRY(d, cur.alloc(gains, d->stream));
+    CUDA_TRY(d, tgt.alloc(gains, d->stream));
+    CUDA_TRY(d, geff.alloc(gains, d->stream));
+    CUDA_TRY(d, gramp.alloc(gains, d->stream));
+    d->d_real_entries = std::move(entries); d->d_real_slot_start = std::move(slotStart);
+    d->d_real_cur = std::move(cur); d->d_real_tgt = std::move(tgt);
+    d->d_real_geff = std::move(geff); d->d_real_gramp = std::move(gramp);
+    return B200MIX_OK;
+}
+
 // Queue tables of the streaming voices (the first voice that reads a queue).
 int ensure_queues(b200mix_device *d)
 {
@@ -297,14 +324,15 @@ int install_slot(b200mix_device *d, uint32_t slot, Fill &&fill)
 static size_t align16(size_t v) { return UploadArena::align(v); }
 
 // b200mix_voices_update's arena: a call packs [VoiceUpdate n][coefficients or directions]
-// [dry gains][send gains] and ships them with one copy.  It holds at least 256 voices.
+// [dry or RealOut gains][send gains] and ships them with one copy.  It holds at least 256 voices,
+// each with room for the wider of the Dry mix's gains and RealOut's (direct-channel voices).
 int ensure_stage(b200mix_device *d, uint32_t n)
 {
     const b200mix_device_desc &dd = d->desc;
     const uint32_t cap = std::max<uint32_t>(n, 256u);
     const size_t bytes = align16(size_t(cap)*sizeof(VoiceUpdate))
         + align16(size_t(cap)*std::max<size_t>(size_t(dd.ir_size)*2, 4)*sizeof(float))
-        + align16(size_t(cap)*dd.dry_channels*sizeof(float))
+        + align16(size_t(cap)*std::max(dd.dry_channels, dd.real_channels)*sizeof(float))
         + align16(size_t(cap)*dd.num_sends*dd.wet_channels*sizeof(float)) + 64;
     CUDA_TRY(d, d->stage.reserve(n, cap, bytes, bytes, d->stream));
     return B200MIX_OK;
@@ -327,7 +355,8 @@ int32_t cb_slot_of(const b200mix_device *d, uint32_t flags, uint32_t buffer)
 // The checks b200mix_voices_update and b200mix_sources_update make of every entry before the call
 // changes anything; `what` prefixes the error.  They may allocate the queue tables and the parked
 // dry bus, which leave the device as it was if they fail.  `nobuf_ok`: the entry may name
-// B200MIX_NO_BUFFER; `hrtf`: the voice mixes through its own HRIR.
+// B200MIX_NO_BUFFER; `hrtf`: the voice does not mix into Dry (it has its own HRIR, or is a
+// direct-channel voice).
 template<typename Entry>
 int check_entry(b200mix_device *d, const char *what, const Entry &p, bool nobuf_ok, bool hrtf)
 {
@@ -373,6 +402,7 @@ ApplyParams apply_params(const b200mix_device *d, const VoiceUpdate *updates)
     A.num_sends = dd.num_sends;
     A.filt = d->d_filt; A.filt_paths = 1u + dd.num_sends;
     A.qhdr = d->d_qhdr;
+    A.real_cur = d->d_real_cur; A.real_tgt = d->d_real_tgt; A.creal = dd.real_channels;
     return A;
 }
 
@@ -402,7 +432,7 @@ extern "C" {
 static void shard_release(b200mix_device *d);
 static int ensure_filters(b200mix_device *d);
 
-uint32_t b200mix_version(void) { return (1u<<16) | 2u; }
+uint32_t b200mix_version(void) { return (1u<<16) | 3u; }
 
 const char *b200mix_last_error(const b200mix_device *dev)
 { return dev ? dev->error.c_str() : g_create_error.c_str(); }
@@ -1151,7 +1181,8 @@ int b200mix_hrtf_attach(b200mix_device *d, const b200mix_hrtf *h)
 }
 
 static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
-    const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains);
+    const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains,
+    bool direct);
 
 // The voices of each callback buffer are the channels of one source: cb_reps[slot] = the first one
 // that mixes this update (-1: none), cb_members[slot] the others, which must agree with it on what
@@ -1183,7 +1214,7 @@ static int cb_group(b200mix_device *d)
 int b200mix_voices_update(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
     const float *hrtf_coeffs, const float *dry_gains, const float *send_gains)
 {
-    return voices_update_impl(d, n, params, hrtf_coeffs, nullptr, dry_gains, send_gains);
+    return voices_update_impl(d, n, params, hrtf_coeffs, nullptr, dry_gains, send_gains, false);
 }
 
 int b200mix_voices_update_dirs(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
@@ -1192,11 +1223,29 @@ int b200mix_voices_update_dirs(b200mix_device *d, uint32_t n, const b200mix_voic
     if(!d) return B200MIX_ERR_INVALID;
     if(!dirs) { d->error = "voices_update_dirs: null directions"; return B200MIX_ERR_INVALID; }
     if(!d->d_st_coeffs) { d->error = "voices_update_dirs: no HRTF data set attached"; return B200MIX_ERR_INVALID; }
-    return voices_update_impl(d, n, params, nullptr, dirs, dry_gains, send_gains);
+    return voices_update_impl(d, n, params, nullptr, dirs, dry_gains, send_gains, false);
 }
 
+int b200mix_voices_update_direct(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
+    const float *real_gains, const float *send_gains)
+{
+    if(!d) return B200MIX_ERR_INVALID;
+    const b200mix_device_desc &dd = d->desc;
+    // where the reference's RealOut.RemixMap is empty (UHJ / TSME) or RealOut is Dry, it never
+    // mixes direct channels (CalcPanningAndFilters, alc/alu.cpp:1535-1599)
+    if(dd.post_process != B200MIX_POST_HRTF && dd.post_process != B200MIX_POST_AMBIDEC)
+    { d->error = "voices_update_direct: the device's output takes no direct channels"; return B200MIX_ERR_UNSUPPORTED; }
+    if(d->shard.world > 1u)
+    { d->error = "voices_update_direct: not on a sharded device set"; return B200MIX_ERR_UNSUPPORTED; }
+    if(d->out.has_stabilizer())
+    { d->error = "voices_update_direct: not with a front stabilizer"; return B200MIX_ERR_UNSUPPORTED; }
+    return voices_update_impl(d, n, params, nullptr, nullptr, real_gains, send_gains, true);
+}
+
+// `direct`: b200mix_voices_update_direct, whose `dry_gains` are RealOut gains.
 static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
-    const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains)
+    const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains,
+    bool direct)
 {
     if(!d) return B200MIX_ERR_INVALID;
     if(n == 0) return B200MIX_OK;
@@ -1206,7 +1255,9 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     for(uint32_t i = 0;i < n;++i)
     {
         const b200mix_voice_params &p = params[i];
-        if(int rc = check_entry(d, "voices_update", p, true, (p.flags & B200MIX_VF_HRTF) != 0)) return rc;
+        if(direct && (p.flags & (B200MIX_VF_DIRECT | B200MIX_VF_HRTF)) != B200MIX_VF_DIRECT)
+        { d->error = "voices_update_direct: every entry has B200MIX_VF_DIRECT and not B200MIX_VF_HRTF"; return B200MIX_ERR_INVALID; }
+        if(int rc = check_entry(d, "voices_update", p, true, direct || (p.flags & B200MIX_VF_HRTF) != 0)) return rc;
         // MaxPitch clamp of the parameter stage (alc/alu.cpp:1682-1685,1996-1999): CalculateBufferSize
         // relies on it
         if(p.step > (10u << 16))
@@ -1222,6 +1273,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         { d->error = "voices_update: a voice starts a callback buffer with B200MIX_VF_RESET"; return B200MIX_ERR_INVALID; }
     }
 
+    if(direct)
+        if(int rc = ensure_real_bus(d)) return rc;
     CUDA_TRY(d, d->stage.wait());
     if(int rc = ensure_stage(d, n)) return rc;
     d->stage.begin();
@@ -1232,7 +1285,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         const bool nobuf = p.buffer == B200MIX_NO_BUFFER;
         const bool stopped = (p.flags & B200MIX_VF_STOPPED) != 0;
         VoiceUpdate &u = upd[i];
-        u.voice = p.voice; u.flags = p.flags; u.buffer = p.buffer; u.resampler = p.resampler;
+        u.voice = p.voice; u.flags = (p.flags & ~kVfDirect) | (direct ? kVfDirect : 0u);
+        u.buffer = p.buffer; u.resampler = p.resampler;
         if(nobuf) { u.flags |= kUpNoBuffer; u.buffer = 0u; }
         u.position = p.position; u.position_frac = p.position_frac;
         u.loop_start = p.loop_start; u.loop_end = p.loop_end; u.step = p.step;
@@ -1246,11 +1300,12 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         for(uint32_t s = 0;s < B200MIX_MAX_SENDS;++s)
             u.send_slot[s] = (s < dd.num_sends) ? p.send_slot[s] : B200MIX_NO_SLOT;
         u.has_coeffs = (hrtf_coeffs != nullptr || (dirs != nullptr && (p.flags & B200MIX_VF_HRTF))) && dd.ir_size > 0;
-        u.has_dry = dry_gains != nullptr;
+        u.has_dry = dry_gains != nullptr && !direct;
         // mixing-order cost key: resampler taps per output
         const uint32_t cost = (p.step == 65536u) ? 1u : (u.bsinc_m ? u.bsinc_m : (p.resampler >= 2u ? 4u : 2u));
         d->book.set(p.voice, {!stopped, cost, (p.flags & B200MIX_VF_HRTF) != 0, p.send_slot,
-            (p.flags & B200MIX_VF_STATIC) && !nobuf ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0});
+            (p.flags & B200MIX_VF_STATIC) && !nobuf ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0,
+            direct});
         if(!d->cbv.empty())
         {
             // the planner's mirror of the voice: what k_apply_updates does to its record
@@ -1284,7 +1339,9 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         apply_dirs(d, A, reinterpret_cast<const float4*>(pack(dirs, size_t(n)*4)));
     else if(hrtf_coeffs && dd.ir_size)
         A.coeffs = pack(hrtf_coeffs, size_t(n)*dd.ir_size*2);
-    if(dry_gains && dd.dry_channels)
+    if(direct && dry_gains && dd.real_channels)
+        A.real = pack(dry_gains, size_t(n)*dd.real_channels);
+    else if(!direct && dry_gains && dd.dry_channels)
         A.dry = pack(dry_gains, size_t(n)*dd.dry_channels);
     if(send_gains && dd.num_sends && dd.wet_channels)
         A.send = pack(send_gains, size_t(n)*dd.num_sends*dd.wet_channels);
@@ -1375,7 +1432,7 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
         uint32_t cost = d->book.cost[p.voice];
         if(bool(d->book.active[p.voice]) != act || (!cost && act)) cost = t ? t->m[0] : (p.resampler >= 2u ? 4u : 2u);
         d->book.set(p.voice, {act, cost, hrtfMode, p.send_slot,
-            (p.flags & B200MIX_VF_STATIC) ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0});
+            (p.flags & B200MIX_VF_STATIC) ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0, false});
     }
     UploadArena &U = d->src;
     U.begin();
@@ -1689,20 +1746,23 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     if(d->cb_bound)
         if(int rc = cb_plan_update(d, frames, cbplan)) return rc;
 
+    VoiceBook &B = d->book;
+    const VoiceBook::Rebuilt re = B.refresh(d->d_filt != nullptr, d->mix_cdr == 0 && d->d_dry_entries,
+        (d->slots.active || force_sends) && d->d_wet && d->d_slot_start);
+    d->real_mixed = !B.real_entries.empty();
+
     stage_mark(d, 0);
     // clear MixBuffer (alc/alu.cpp:2417) and the wet buffers (alc/alu.cpp:2196-2198)
     // (the dry mix is left alone while nothing can write or read it: HRTF-only scenes; an
-    // HRTF post-process whose RealOut is just L/R overwrites it instead of accumulating)
+    // HRTF post-process whose RealOut is just L/R overwrites it instead of accumulating, unless
+    // the RealOut bus has mixed direct-channel voices into it)
     if(d->book.dry_active || dd.post_process != B200MIX_POST_HRTF)
         CUDA_TRY(d, cudaMemsetAsync(d->d_dry, 0, size_t(d->dry_alloc_ch)*kLine*sizeof(float), d->stream));
-    if(d->d_real != d->d_dry && !d->out.overwrites_real())
+    if(d->d_real != d->d_dry && (!d->out.overwrites_real() || d->real_mixed))
         CUDA_TRY(d, cudaMemsetAsync(d->d_real, 0, size_t(dd.real_channels)*kLine*sizeof(float), d->stream));
     if(d->d_wet)
         CUDA_TRY(d, cudaMemsetAsync(d->d_wet, 0, size_t(dd.max_slots)*dd.wet_channels*kLine*sizeof(float), d->stream));
 
-    VoiceBook &B = d->book;
-    const VoiceBook::Rebuilt re = B.refresh(d->d_filt != nullptr, d->mix_cdr == 0 && d->d_dry_entries,
-        (d->slots.active || force_sends) && d->d_wet && d->d_slot_start);
     if(re.order)
         if(int rc = upload(d, d->d_order, B.order)) return rc;
     if(re.order2)
@@ -1717,6 +1777,12 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     {
         if(int rc = upload(d, d->d_slot_start, B.slot_start)) return rc;
         if(int rc = upload(d, d->d_entries, B.entries)) return rc;
+    }
+    if(re.real && d->d_real_entries)
+    {
+        const uint32_t ss[2] = {0u, uint32_t(B.real_entries.size())};
+        CUDA_TRY(d, cudaMemcpyAsync(d->d_real_slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, d->stream));
+        if(int rc = upload(d, d->d_real_entries, B.real_entries)) return rc;
     }
     const uint32_t numOrder = uint32_t(B.order.size()), numOrder2 = uint32_t(B.order2.size());
     const uint32_t numDry = uint32_t(B.dry_entries.size()), numEntries = uint32_t(B.entries.size());
@@ -1830,6 +1896,20 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
                 && frames == uint32_t(kLine) && chunks > 1u;
             if(int rc = run_bus_mix(d, DM, numDry, 1u, tc)) return rc;
         }
+    }
+
+    // ---- RealOut bus: direct-channel voices (core/voice.cpp:947-963 with mDirect.Buffer = RealOut)
+    // in index order, one pseudo slot of real_channels; RealOut is then (direct sum) + the
+    // post-process' output, the reference's association ----
+    if(d->real_mixed)
+    {
+        SendMixParams RM{};
+        RM.slot_start = d->d_real_slot_start; RM.entries = d->d_real_entries; RM.sendinfo = d->d_sendinfo;
+        RM.xscratch = d->d_xscratch; RM.send_cur = d->d_real_cur; RM.send_tgt = d->d_real_tgt;
+        RM.wet = d->d_real; RM.frames = frames; RM.cw = dd.real_channels; RM.num_sends = 1;
+        RM.valid_bit = kSiReal; RM.dline = d->d_dline ? d->d_dline : d->d_xscratch;
+        RM.chunks = 1; RM.geff = d->d_real_geff; RM.gramp = d->d_real_gramp;
+        if(int rc = run_bus_mix(d, RM, uint32_t(B.real_entries.size()), 1u, false)) return rc;
     }
 
     stage_mark(d, 5);
@@ -1948,8 +2028,8 @@ static int render_phase_b(b200mix_device *d, uint32_t frames)
     }
 
     stage_mark(d, 7);
-    if(int rc = d->out.post(d->d_dry, d->d_real, d->d_partial, d->fir_rows, d->book.dry_active, d->fir_done,
-        frames, d->launches)) return rc;
+    if(int rc = d->out.post(d->d_dry, d->d_real, d->d_partial, d->fir_rows, d->book.dry_active, d->real_mixed,
+        d->fir_done, frames, d->launches)) return rc;
     stage_mark(d, 8);
     if(d->profile_level >= 2) d->stage_valid = true;
     CUDA_TRY(d, cudaGetLastError());
@@ -2104,6 +2184,8 @@ int b200mix_set_uhj_encoder(b200mix_device *d, uint32_t filter_length, uint32_t 
 
 int b200mix_set_front_stabilizer(b200mix_device *d, uint32_t center_channel, float splitter_coeff)
 {
+    if(d && center_channel != B200MIX_NO_SLOT && d->book.has_direct())
+    { d->error = "set_front_stabilizer: not with active direct-channel voices"; return B200MIX_ERR_UNSUPPORTED; }
     return set_output(d, "set_front_stabilizer", &OutputStage::set_front_stabilizer, center_channel, splitter_coeff);
 }
 
@@ -2192,6 +2274,9 @@ static int shard_common(b200mix_device *d, uint32_t rank, uint32_t world)
     if(world < 1u || world > kShardMaxWorld || rank >= world)
     { d->error = "shard: rank/world out of range (world <= 16)"; return B200MIX_ERR_INVALID; }
     if(d->mid_render) { d->error = "shard: a render_begin is pending"; return B200MIX_ERR_INVALID; }
+    // a sharded set has no RealOut bus (b200mix_voices_update_direct refuses it)
+    if(world > 1u && d->book.has_direct())
+    { d->error = "shard: not with active direct-channel voices"; return B200MIX_ERR_UNSUPPORTED; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     CUDA_TRY(d, cudaStreamSynchronize(d->stream));
     shard_release(d);

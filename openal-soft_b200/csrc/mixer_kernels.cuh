@@ -112,10 +112,11 @@ struct MixParams {
 
 constexpr uint32_t kMaxQueue = 32, kNoLoop = 0xffffffffu;
 
-// sendinfo bits: the line is parked for the aux sends (kSiSend), the parked dry bus (kSiDry)
-// or k_hrtf_fir (kSiHrtf); kSiDeferred: its direct filter is active, the mix reads dline
+// sendinfo bits: the line is parked for the aux sends (kSiSend), the parked dry bus (kSiDry),
+// k_hrtf_fir (kSiHrtf) or the RealOut bus (kSiReal: a direct-channel voice); kSiDeferred: its
+// direct filter is active, the mix reads dline
 constexpr uint32_t kSiSend = 1u, kSiPlaying = 2u, kSiDeferred = 4u, kSiDirty = 8u, kSiDry = 16u,
-    kSiHrtf = 32u;
+    kSiHrtf = 32u, kSiReal = 64u;
 
 // Named barrier of voice group id (1 or 2).  The ids are immediates: with a register id ptxas
 // reserves all 16 hardware barriers for the CTA, which caps the SM at 4 such CTAs.
@@ -937,20 +938,22 @@ __device__ __forceinline__ void advance_chunk(float *win, float *prev, bool pack
 // HRTF devices, or more than 4 dry channels) mixes no voice itself: every line is parked, HRTF
 // voices for k_hrtf_fir (kSiHrtf), the others for k_send_mix, which sums the dry bus like one
 // more slot (kSiDry; deterministic, no atomics).  sendinfo carries what those kernels need of
-// the voice's state.
+// the voice's state.  A direct-channel voice's line is parked for the RealOut bus (kSiReal) by
+// both variants.
 template<int GS, int CDR>
 __device__ __forceinline__ void park_voice(const MixParams &P, const float *xs, uint32_t v,
-    uint32_t sendMask, bool defer, bool isHrtf, bool playing, bool dirty, uint32_t counter, int t)
+    uint32_t sendMask, bool defer, bool isHrtf, bool isDirect, bool playing, bool dirty, uint32_t counter, int t)
 {
     const uint32_t n = P.frames;
     const bool sends = P.num_sends && sendMask;
-    const bool park = sends || defer || CDR == 0;
+    const bool park = sends || defer || isDirect || CDR == 0;
     if(CDR > 0 && park)
         for(uint32_t k = t;k < n;k += GS) P.xscratch[size_t(v)*kLine + k] = xs[k];
     if(t == 0)
         P.sendinfo[v] = park ? ((sends ? kSiSend : 0u)
             | (playing ? kSiPlaying : 0u) | (defer ? kSiDeferred : 0u) | (dirty ? kSiDirty : 0u)
-            | ((CDR == 0 && !isHrtf) ? kSiDry : 0u) | (isHrtf ? kSiHrtf : 0u) | (counter << 8)) : 0u;
+            | ((CDR == 0 && !isHrtf && !isDirect) ? kSiDry : 0u) | (isHrtf ? kSiHrtf : 0u)
+            | (isDirect ? kSiReal : 0u) | (counter << 8)) : 0u;
 }
 
 // MixSamples -> Mix_ (core/mixer.h:27-41, mixer_c.cpp:150-186,247-258) of one line into the
@@ -1176,6 +1179,8 @@ k_mix_voices(const MixParams P)
         // mixed through its own HRIR by k_hrtf_fir (HRTF devices only)
         const bool isHrtf = CDR == 0 && P.ir_pad != 0u && (flags & kVfHrtf);
         const bool dirty = (flags & kVfCoefDirty) != 0;
+        // mixed into RealOut by the RealOut bus (never HRTF: the host refuses both)
+        const bool isDirect = (flags & kVfDirect) != 0;
         FilterRec *dfilt = P.filt ? P.filt + size_t(v)*P.filt_paths : nullptr;
         // a voice with an active direct filter is only resampled here; its mix is deferred
         const bool defer = dfilt && dfilt->active;
@@ -1252,11 +1257,11 @@ k_mix_voices(const MixParams P)
         // the send mask is read here rather than held through the chunks: the parking
         // variant has no register to spare there
         if(P.sendinfo)
-            park_voice<GS, CDR>(P, xs, v, rec.send_mask, defer, isHrtf, playing, dirty, counter, t);
+            park_voice<GS, CDR>(P, xs, v, rec.send_mask, defer, isHrtf, isDirect, playing, dirty, counter, t);
         // direct-path DoFilters (core/voice.cpp:943-946) with an inactive pair: clear()
         if(dfilt && !defer) filter_clear(*dfilt, t);
         if constexpr(CDR > 0)
-            if(!defer)
+            if(!defer && !isDirect)
                 mix_dry<GS, CDR>(accD, xs, S.newGain, P.dry_cur + size_t(v)*P.cd, P.dry_tgt + size_t(v)*P.cd,
                     P.cd, n, counter, playing, t);
         // a callback voice's span ends where its stored samples do: the static end check is
@@ -1265,7 +1270,7 @@ k_mix_voices(const MixParams P)
             write_back_voice(P, rec, v, h1, flags, vstate, increment, haveBuffer, isQueue, qh, qitems,
                 looping, loopStart, loopEnd, buf.frames);
         group_sync(bar, GS);               // smem free for the next voice
-        if(CDR > 0 && !defer) store_dry_gains(P.dry_cur + size_t(v)*P.cd, S.newGain, P.cd, t);
+        if(CDR > 0 && !defer && !isDirect) store_dry_gains(P.dry_cur + size_t(v)*P.cd, S.newGain, P.cd, t);
         group_sync(bar, GS);
     }
 
@@ -1281,7 +1286,8 @@ k_mix_voices(const MixParams P)
 
 // ---------------------------------------------------------------------------
 // The deferred dry pass (register-dry devices).  Mixes the voices k_mix_voices parked with
-// kSiDeferred once k_filters has left their filtered line in dline.  Same static assignment
+// kSiDeferred (direct-channel voices, kSiReal, excepted: the RealOut bus mixes them) once
+// k_filters has left their filtered line in dline.  Same static assignment
 // over the order it is given (order2), the same Mix_ arithmetic and the same partial-row
 // combine as k_mix_voices<GS,GROUPS,CDR>, so the sums and their order are unchanged.
 // ---------------------------------------------------------------------------
@@ -1314,7 +1320,7 @@ k_mix_deferred(const MixParams P)
     {
         const uint32_t v = P.order[oi];
         const uint32_t info = P.sendinfo[v];
-        if(!(info & kSiDeferred)) continue;
+        if((info & (kSiDeferred | kSiReal)) != kSiDeferred) continue;
         const float *fl = P.dline + size_t(v)*kLine;
         for(uint32_t k = t;k < n;k += GS) S.x[k] = fl[k];
         group_sync(bar, GS);               // line staged
@@ -1677,6 +1683,9 @@ struct ApplyParams {
     const uint8_t *st_delays;    // [ir_count][2]
     uint32_t st_num_fields, st_ir;
     uint4 *qhdr;                 // streaming queues (null: none): a restart rewinds the head
+    // direct-channel voices (null until the first b200mix_voices_update_direct): staged RealOut
+    // gains [n][creal], Current / Target [max_voices][creal]
+    const float *real; float *real_cur, *real_tgt; uint32_t creal;
 };
 
 // HrtfStore::getCoeffs (core/hrtf.cpp:192-260) on the device, in the exact operation order of
@@ -1827,6 +1836,7 @@ __global__ void __launch_bounds__(64) k_apply_updates(const ApplyParams A)
         if(A.send_cur)
             for(uint32_t c = t;c < A.num_sends*A.cw;c += 64)
                 A.send_cur[size_t(up.voice)*A.num_sends*A.cw + c] = 0.0f;
+        if(A.real_cur) for(uint32_t c = t;c < A.creal;c += 64) A.real_cur[size_t(up.voice)*A.creal + c] = 0.0f;
         if(A.filt)          // chandata.mDryParams = DirectParams{}; mWetParams = SendParams{} (voice.cpp:1387-1394)
             for(uint32_t k = t;k < A.filt_paths*32u;k += 64)
                 filter_reset_word(A.filt + size_t(up.voice)*A.filt_paths + (k >> 5), int(k & 31u));
@@ -1870,12 +1880,28 @@ __global__ void __launch_bounds__(64) k_apply_updates(const ApplyParams A)
     if(up.has_dry && A.dry_tgt)
         for(uint32_t c = t;c < A.cd;c += 64)
             A.dry_tgt[size_t(up.voice)*A.cd + c] = A.dry[size_t(u)*A.cd + c];
+    // The reference's voice has one mDryParams.Gains.Current, indexed by the channels of whichever
+    // buffer its direct path feeds: a voice moved between Dry and RealOut carries the shared
+    // channel indices' Current gains across; the others keep what they had.
+    if(!reset && A.real_cur && ((oldFlags ^ up.flags) & kVfDirect))
+    {
+        float *dc = A.dry_cur + size_t(up.voice)*A.cd, *rc = A.real_cur + size_t(up.voice)*A.creal;
+        const bool toReal = (up.flags & kVfDirect) != 0;
+        for(uint32_t c = t;c < min(A.cd, A.creal);c += 64)
+        {
+            if(toReal) rc[c] = dc[c];
+            else dc[c] = rc[c];
+        }
+    }
+    if(A.real)
+        for(uint32_t c = t;c < A.creal;c += 64)
+            A.real_tgt[size_t(up.voice)*A.creal + c] = A.real[size_t(u)*A.creal + c];
     if(A.send && A.send_tgt)
         for(uint32_t c = t;c < A.num_sends*A.cw;c += 64)
             A.send_tgt[size_t(up.voice)*A.num_sends*A.cw + c] = A.send[size_t(u)*A.num_sends*A.cw + c];
     if(t == 0)
     {
-        uint32_t fl = up.flags & (kVfStatic|kVfLooping|kVfHrtf|kVfChannelMask);
+        uint32_t fl = up.flags & (kVfStatic|kVfLooping|kVfHrtf|kVfChannelMask|kVfDirect);
         if(reset)
         {
             rec.pos = up.position; rec.frac = up.position_frac;
@@ -2331,7 +2357,10 @@ __global__ void __launch_bounds__(1024) k_post_stabilizer(const StabParams Q)
 // thread each on its own warp, inputs and outputs staged in shared memory; operations in the
 // reference's order with explicit rounding.  coef = {a0_lo, b1_lo, a0_hi, a1_hi, b1_hi},
 // state = history[2]{lo, hi}.
-struct Bs2bParams { float *real; float *state; const float *coef; uint32_t frames, real_left, real_right; };
+// `direct` (null: none): the direct-channel signal of L/R [2][1024], moved out of RealOut before
+// the decode and added back after the cross-feed (alc/alu.cpp:414-433).
+struct Bs2bParams { float *real; float *state; const float *coef; uint32_t frames, real_left, real_right;
+    const float *direct; };
 
 __global__ void __launch_bounds__(128) k_post_bs2b(const Bs2bParams Q)
 {
@@ -2379,6 +2408,12 @@ __global__ void __launch_bounds__(128) k_post_bs2b(const Bs2bParams Q)
         left[k] = __fadd_rn(sOut[0][k], sOut[2][k]);
         right[k] = __fadd_rn(sOut[1][k], sOut[3][k]);
     }
+    if(Q.direct)
+        for(uint32_t k = threadIdx.x;k < n;k += blockDim.x)
+        {
+            left[k] = __fadd_rn(left[k], Q.direct[k]);
+            right[k] = __fadd_rn(right[k], Q.direct[kLine + k]);
+        }
 }
 
 // UhjEncoder<N>::encode (core/uhjfilter.cpp:83-205), N = 256 or 512.  The reference shifts

@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(64) k_calc_voices(const CalcVoicesParams Q)
 
     VoiceUpdate u;
     u.voice = sv.voice; u.buffer = sv.buffer; u.resampler = sv.resampler;
-    u.flags = (sv.flags & ~uint32_t(B200MIX_VF_HRTF)) | (is_hrtf ? uint32_t(B200MIX_VF_HRTF) : 0u);
+    u.flags = (sv.flags & ~uint32_t(B200MIX_VF_HRTF | kVfDirect)) | (is_hrtf ? uint32_t(B200MIX_VF_HRTF) : 0u);
     if(!ok) u.flags = (u.flags & ~3u) | uint32_t(B200MIX_VF_STOPPED);      // a bad mix map: silence the voice
     u.position = sv.position; u.position_frac = sv.position_frac;
     u.loop_start = sv.loop_start; u.loop_end = sv.loop_end;

@@ -5,7 +5,9 @@
 //   order2        the voices of `order` with an active direct filter (all of them once the GPU
 //                 parameter stage decides filter activity: k_filters and k_mix_deferred then look
 //                 at every voice's kSiDeferred bit)
-//   dry_entries   the active non-HRTF voices in index order (the parked dry bus)
+//   dry_entries   the active voices that mix into Dry (neither HRTF nor direct) in index order
+//                 (the parked dry bus)
+//   real_entries  the active direct-channel voices in index order (the RealOut bus)
 //   slot_start / entries   per slot, its (voice, send) pairs: voices, then sends, in index order
 // The setters mark the lists a change affects; refresh() rebuilds those and says which, for the
 // caller to upload.  Host code only.
@@ -22,12 +24,14 @@ namespace b200mix {
 struct VoiceBook {
     // One voice as an update leaves it: active (not B200MIX_VF_STOPPED), its mixing-order cost key
     // (resampler taps per output), HRTF (mixes through its own HRIR, not the dry bus), its aux slot
-    // per send, the static buffer it plays (or B200MIX_NO_SLOT), RESET (clears the direct filter).
-    struct State { bool active; uint32_t cost; bool hrtf; const uint32_t *send_slot; uint32_t buffer; bool reset; };
-    struct Rebuilt { bool order, order2, dry, sends; };
+    // per send, the static buffer it plays (or B200MIX_NO_SLOT), RESET (clears the direct filter),
+    // DIRECT (mixes into RealOut, not the dry bus).
+    struct State { bool active; uint32_t cost; bool hrtf; const uint32_t *send_slot; uint32_t buffer; bool reset;
+        bool direct; };
+    struct Rebuilt { bool order, order2, dry, sends, real; };
 
     uint32_t num_sends{0}, max_slots{0};
-    std::vector<uint8_t> active, hrtf, dfilt;      // dfilt: direct filter active
+    std::vector<uint8_t> active, hrtf, dfilt, direct;   // dfilt: direct filter active
     std::vector<uint32_t> cost, vbuf;              // vbuf: static buffer an active voice plays
     std::vector<uint32_t> send_slot;               // [voice][num_sends]
     std::vector<uint32_t> bufrefs;                 // active static voices per buffer
@@ -36,14 +40,15 @@ struct VoiceBook {
     bool dev_filters{false};                       // filter activity is decided on the device
 
     std::vector<uint32_t> order, order2, slot_start;
-    std::vector<SendEntry> dry_entries, entries;
+    std::vector<SendEntry> dry_entries, entries, real_entries;
     uint32_t max_slot_entries{0};
-    bool order_dirty{true}, order2_dirty{false}, dry_dirty{true}, sends_dirty{true};
+    bool order_dirty{true}, order2_dirty{false}, dry_dirty{true}, sends_dirty{true}, real_dirty{false};
 
     void init(uint32_t max_voices, uint32_t max_buffers, uint32_t sends, uint32_t slots)
     {
         num_sends = sends; max_slots = slots;
         active.assign(max_voices, 0); hrtf.assign(max_voices, 0); dfilt.assign(max_voices, 0);
+        direct.assign(max_voices, 0);
         cost.assign(max_voices, 0); vbuf.assign(max_voices, B200MIX_NO_SLOT);
         send_slot.assign(size_t(max_voices)*num_sends, B200MIX_NO_SLOT);
         bufrefs.assign(std::max(max_buffers, 1u), 0u);
@@ -57,9 +62,11 @@ struct VoiceBook {
             const uint32_t slot = s.active ? s.send_slot[k] : B200MIX_NO_SLOT;
             if(m != slot) { m = slot; sends_dirty = true; }
         }
-        if(s.active && !s.hrtf) dry_active = true;
+        if(s.active && !s.hrtf && !s.direct) dry_active = true;
         if(hrtf[v] != s.hrtf) { hrtf[v] = s.hrtf; dry_dirty = true; }
+        if(direct[v] != s.direct) { direct[v] = s.direct; dry_dirty = real_dirty = true; }
         if(active[v] != s.active || cost[v] != s.cost) order_dirty = true;
+        if(direct[v] && active[v] != s.active) real_dirty = true;
         active[v] = s.active; cost[v] = s.cost;
         voice_hi = std::max(voice_hi, v + 1u);
         const uint32_t nb = s.active ? s.buffer : B200MIX_NO_SLOT;
@@ -71,14 +78,19 @@ struct VoiceBook {
         }
         if(s.reset) set_direct_filter(v, false);
     }
+    bool has_direct() const
+    {
+        for(uint32_t v = 0;v < voice_hi;++v) if(active[v] && direct[v]) return true;
+        return false;
+    }
     void set_direct_filter(uint32_t v, bool on) { if(dfilt[v] != on) { dfilt[v] = on; order2_dirty = true; } }
     void set_device_filters() { order2_dirty |= !dev_filters; dev_filters = true; }
 
     // order2 is kept once the device has filters, the dry entries once it parks its dry bus, the
-    // send CSR while it mixes sends.
+    // send CSR while it mixes sends; the RealOut entries whenever a direct voice changes.
     Rebuilt refresh(bool filters, bool dry, bool sends)
     {
-        Rebuilt r{order_dirty, false, false, false};
+        Rebuilt r{order_dirty, false, false, false, real_dirty};
         if(r.order)
         {
             order.clear();
@@ -96,8 +108,15 @@ struct VoiceBook {
         if(r.dry)
         {
             dry_entries.clear();
-            for(uint32_t v = 0;v < voice_hi;++v) if(active[v] && !hrtf[v]) dry_entries.push_back(SendEntry{v, 0u});
+            for(uint32_t v = 0;v < voice_hi;++v)
+                if(active[v] && !hrtf[v] && !direct[v]) dry_entries.push_back(SendEntry{v, 0u});
             dry_dirty = false;
+        }
+        if(r.real)
+        {
+            real_entries.clear();
+            for(uint32_t v = 0;v < voice_hi;++v) if(active[v] && direct[v]) real_entries.push_back(SendEntry{v, 0u});
+            real_dirty = false;
         }
         if(r.sends)
         {

@@ -40,6 +40,10 @@ struct SlotRec {
 
 constexpr int kMaxSends = 6;
 
+// VoiceUpdate / VoiceRec flag of a direct-channel voice (direct path RealOut); set by
+// b200mix_voices_update_direct only, never taken from the caller's flags.
+constexpr uint32_t kVfDirect = 1u<<12;
+
 struct alignas(16) VoiceUpdate {   // staged by b200mix_voices_update
     uint32_t voice, flags, buffer, resampler;
     int32_t  position; uint32_t position_frac, loop_start, loop_end;
