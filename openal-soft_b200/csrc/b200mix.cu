@@ -29,11 +29,11 @@
 #include "resampler_tables.hpp"
 #include "hrtf_store.hpp"
 #include "adpcm.hpp"
-#include "callback_plan.hpp"
 #include "device_memory.hpp"
 #include "voice_book.hpp"
 #include "slot_table.hpp"
 #include "output_stage.hpp"
+#include "buffer_table.hpp"
 
 using namespace b200mix;
 
@@ -56,9 +56,8 @@ struct b200mix_device {
     DevArray<float> d_bsinc[3], d_cubic[2];
 
     // state
-    DevArray<VoiceRec> d_voices; DevArray<BufferRec> d_buffers;
-    std::vector<BufferRec> h_buffers;
-    std::vector<DevArray<char>> buf_store;       // per buffer: the samples its h_buffers record views
+    DevArray<VoiceRec> d_voices;
+    BufferTable buffers;                          // buffers and callback buffers, source of the device's records
     VoiceBook book;                               // host mirror of the voices, source of d_order & co.
     DevArray<uint32_t> d_order;                   // book.order
     DevArray<float2> d_hrtf_tgt, d_hrtf_old;
@@ -149,35 +148,8 @@ struct b200mix_device {
     int fir_blocks_per_sm{0};        // k_hrtf_fir CTAs per SM (HRTF devices)
     uint64_t fir_done{0};            // `launches` once the last update's k_hrtf_fir was launched
 
-    // callback buffers (b200mix_buffer_callback): the registrations (plan slots), the host's
-    // mirror of the voices that play them (positions advance by the same arithmetic as on the
-    // device, so planning needs no read-back), and the pinned arenas their samples travel in,
-    // alternating so that one can be filled while the other's copy is in flight
-    struct CbBuf {
-        bool used{false};
-        uint32_t buffer{0};
-        b200mix_callback_buffer cb{};
-        cbplan::State st{};
-        uint32_t frame_bytes{0};             // bytes per sample frame in the arena (int16 for ADPCM)
-    };
-    std::vector<CbBuf> cbs;
-    std::vector<int32_t> cb_of_buffer;       // buffer id -> plan slot or -1
-    struct CbVoice { int32_t slot{-1}; cbplan::Voice v{}; };
-    std::vector<CbVoice> cbv;                // per voice
-    uint32_t cb_bound{0};                    // voices bound to a callback buffer
-    UploadArena cb_arena[2]; int cb_idx{0};
-    DevArray<char> d_cb_zero;                // zeros behind every callback buffer's own record
-    std::vector<int32_t> cb_reps;            // per slot: the voice the update is planned from (-1: none)
-    std::vector<std::vector<uint32_t>> cb_members;   // per slot: its other mixing voices
-    struct CbWork { cbplan::State start; cbplan::Loads loads; size_t region{0}, bytes{0}; };
-    std::vector<CbWork> cb_work;             // per slot, for the update being planned
     ~b200mix_device() { if(stream) cudaStreamDestroy(stream); }
 };
-
-namespace {
-constexpr uint32_t kCbMaxChannels = 16;      // a callback buffer's frame is at most 16*8 bytes
-constexpr size_t kCbPad = 256;               // zero bytes that cover one such frame
-}
 
 namespace {
 
@@ -345,13 +317,6 @@ const BsincTable *bsinc_for(const b200mix_device *d, uint32_t resampler)
     return &d->bsinc[(resampler - B200MIX_RESAMPLER_FAST_BSINC12) >> 1];
 }
 
-// Plan slot of the callback buffer an entry plays (-1: none).
-int32_t cb_slot_of(const b200mix_device *d, uint32_t flags, uint32_t buffer)
-{
-    return (!(flags & B200MIX_VF_STOPPED) && buffer != B200MIX_NO_BUFFER && !d->cb_of_buffer.empty())
-        ? d->cb_of_buffer[buffer] : -1;
-}
-
 // The checks b200mix_voices_update and b200mix_sources_update make of every entry before the call
 // changes anything; `what` prefixes the error.  They may allocate the queue tables and the parked
 // dry bus, which leave the device as it was if they fail.  `nobuf_ok`: the entry may name
@@ -370,14 +335,10 @@ int check_entry(b200mix_device *d, const char *what, const Entry &p, bool nobuf_
     if((p.flags & B200MIX_VF_LOOPING) && p.loop_end <= p.loop_start)
         return bad("empty loop");
     // nothing to read without a buffer; a callback voice reads from the update's arena
-    if(!stopped && !nobuf && cb_slot_of(d, p.flags, p.buffer) < 0)
+    if(!stopped && !nobuf && d->buffers.cb_slot(p.flags, p.buffer) < 0)
     {
         if(p.flags & B200MIX_VF_STATIC)
-        {
-            const BufferRec &hb = d->h_buffers[p.buffer];
-            if(!hb.data || !hb.frames) return bad("static voice on a buffer without data");
-            if((p.flags & B200MIX_VF_LOOPING) && p.loop_end > hb.frames) return bad("loop end beyond the buffer");
-        }
+        { if(const char *why = d->buffers.unplayable_static(p.buffer, (p.flags & B200MIX_VF_LOOPING) ? p.loop_end : 0u)) return bad(why); }
         // a streaming voice reads its queue: make sure the (empty) queue table exists
         else if(int rc = ensure_queues(d)) return rc;
     }
@@ -423,6 +384,16 @@ int set_output(b200mix_device *d, const char *what, int (OutputStage::*set)(Para
     if(d->mid_render) { d->error = std::string(what) + ": a render_begin is pending"; return B200MIX_ERR_INVALID; }
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     return (d->out.*set)(args...);
+}
+
+// Every buffer setter: on the mixer's GPU, the table checks the call against the buffers the voices
+// hold, then builds and commits the new state (BufferTable).
+template<typename... Params, typename... Args>
+int set_buffer(b200mix_device *d, int (BufferTable::*set)(Params...), Args... args)
+{
+    if(!d) return B200MIX_ERR_INVALID;
+    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
+    return (d->buffers.*set)(args..., d->book.bufrefs);
 }
 
 } // namespace
@@ -492,9 +463,7 @@ int b200mix_create(const b200mix_device_desc *desc, b200mix_device **out)
         const b200mix_device_desc &dd = d->desc;
         d->ir_pad = (dd.ir_size + 7u) & ~7u;
         CUDA_TRY(d, d->d_voices.alloc(dd.max_voices, d->stream));
-        CUDA_TRY(d, d->d_buffers.alloc(std::max(dd.max_buffers, 1u), d->stream));
-        d->h_buffers.assign(std::max(dd.max_buffers, 1u), BufferRec{});
-        d->buf_store.resize(d->h_buffers.size());
+        if(int rc = d->buffers.init(dd.max_buffers, dd.max_voices, d->stream, d->error)) return rc;
         d->book.init(dd.max_voices, dd.max_buffers, dd.num_sends, dd.max_slots);
         if(dd.ir_size)
         {
@@ -636,137 +605,16 @@ int b200mix_set_ambi_decoder(b200mix_device *d, uint32_t in_channels, const floa
         xover_coeff);
 }
 
-// Voices that play callback plan slot s (playing or stopping).
-static uint32_t cb_slot_voices(const b200mix_device *d, int32_t s)
-{
-    uint32_t n = 0;
-    for(uint32_t v = 0;v < d->cbv.size() && v < d->book.voice_hi;++v)
-        n += d->cbv[v].slot == s && (d->cbv[v].v.state == 1u || d->cbv[v].v.state == 2u);
-    return n;
-}
-
-// Ends the callback registration of `buffer` (if any); refused while a voice plays it.
-static int cb_unregister(b200mix_device *d, uint32_t buffer, const char *what)
-{
-    if(d->cb_of_buffer.empty() || d->cb_of_buffer[buffer] < 0) return B200MIX_OK;
-    const int32_t s = d->cb_of_buffer[buffer];
-    if(cb_slot_voices(d, s))
-    { d->error = std::string(what) + ": the callback buffer is played by a voice; stop it first"; return B200MIX_ERR_INVALID; }
-    for(auto &cv : d->cbv)
-        if(cv.slot == s) { cv.slot = -1; --d->cb_bound; }
-    d->cbs[size_t(s)] = b200mix_device::CbBuf{};
-    d->cb_of_buffer[buffer] = -1;
-    d->h_buffers[buffer] = BufferRec{};
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &d->h_buffers[buffer], sizeof(BufferRec),
-        cudaMemcpyHostToDevice, d->stream));
-    return B200MIX_OK;
-}
-
 int b200mix_buffer_callback(b200mix_device *d, uint32_t buffer, const b200mix_callback_buffer *cb)
-{
-    if(!d) return B200MIX_ERR_INVALID;
-    const b200mix_device_desc &dd = d->desc;
-    if(buffer >= dd.max_buffers || !cb || cb->struct_size != sizeof(b200mix_callback_buffer) || !cb->callback
-        || cb->sample_type > B200MIX_FMT_MSADPCM || cb->channels < 1 || !cb->storage
-        || cb->samples_per_block < 1 || cb->bytes_per_block < 1)
-    { d->error = "buffer_callback: bad arguments"; return B200MIX_ERR_INVALID; }
-    static const uint32_t sz[] = {1, 2, 4, 4, 8, 1, 1};
-    const bool adpcm = cb->sample_type >= B200MIX_FMT_IMA4;
-    const bool ms = cb->sample_type == B200MIX_FMT_MSADPCM;
-    if(adpcm ? (cb->channels > 2 || !AdpcmBlockValid(ms, cb->samples_per_block)
-                || cb->bytes_per_block != AdpcmBlockBytes(ms, cb->channels, cb->samples_per_block))
-             : (cb->samples_per_block != 1u || cb->bytes_per_block != cb->channels*sz[cb->sample_type]))
-    { d->error = "buffer_callback: block size does not match the format"; return B200MIX_ERR_INVALID; }
-    if(cb->channels > kCbMaxChannels)
-    { d->error = "buffer_callback: more than 16 channels"; return B200MIX_ERR_UNSUPPORTED; }
-    // PrepareCallback's size (al/buffer.cpp:468-473): MixerLineSize*MaxPitch + MaxResamplerEdge
-    // samples in whole blocks.  No request of the reference's chunk loop passes it, so the
-    // callbacks of an update never stop half way.
-    const uint64_t lineBlocks = ((1024u + 256u)*10u + 24u + cb->samples_per_block - 1u) / cb->samples_per_block;
-    if(cb->storage_bytes < lineBlocks*cb->bytes_per_block)
-    { d->error = "buffer_callback: storage smaller than the reference's callback storage"; return B200MIX_ERR_INVALID; }
-    if(uint64_t(cb->num_blocks)*cb->bytes_per_block > cb->storage_bytes || cb->stopped > 1u)
-    { d->error = "buffer_callback: state outside the storage"; return B200MIX_ERR_INVALID; }
-    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(!d->d_cb_zero)
-        CUDA_TRY(d, d->d_cb_zero.alloc(kCbPad, d->stream));
-    if(d->cb_of_buffer.empty())
-    {
-        d->cb_of_buffer.assign(dd.max_buffers, -1);
-        d->cbv.assign(dd.max_voices, b200mix_device::CbVoice{});
-    }
-    BufferRec &h = d->h_buffers[buffer];
-    int32_t s = d->cb_of_buffer[buffer];
-    if(s < 0)
-    {
-        if(h.data && d->book.bufrefs[buffer])
-        { d->error = "buffer_callback: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
-        if(h.data)
-        {
-            CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-            d->buf_store[buffer].reset();
-        }
-        for(s = 0;size_t(s) < d->cbs.size() && d->cbs[size_t(s)].used;++s) {}
-        if(size_t(s) == d->cbs.size()) d->cbs.emplace_back();
-        d->cb_of_buffer[buffer] = s;
-    }
-    b200mix_device::CbBuf &c = d->cbs[size_t(s)];
-    c.used = true; c.buffer = buffer; c.cb = *cb;
-    c.st = cbplan::State{cb->num_blocks, cb->block_offset, cb->stopped};
-    c.frame_bytes = cb->channels*(adpcm ? 2u : sz[cb->sample_type]);
-    // the kernel reads the samples from the update's arena: the record carries the format, and
-    // zeros to read should a voice ever meet it without a plan
-    h = BufferRec{};
-    h.data = d->d_cb_zero.get();
-    h.type = adpcm ? uint32_t(B200MIX_FMT_I16) : cb->sample_type;
-    h.channels = cb->channels;
-    h.pad = uint32_t(s) + 1u;
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec), cudaMemcpyHostToDevice, d->stream));
-    return B200MIX_OK;
-}
+{ return set_buffer(d, &BufferTable::set_callback, buffer, cb); }
 
 int b200mix_buffer_callback_state(b200mix_device *d, uint32_t buffer, uint32_t *num_blocks,
     uint32_t *block_offset, uint32_t *stopped)
-{
-    if(!d) return B200MIX_ERR_INVALID;
-    if(buffer >= d->desc.max_buffers || d->cb_of_buffer.empty() || d->cb_of_buffer[buffer] < 0)
-    { d->error = "buffer_callback_state: not a callback buffer"; return B200MIX_ERR_INVALID; }
-    const cbplan::State &st = d->cbs[size_t(d->cb_of_buffer[buffer])].st;
-    if(num_blocks) *num_blocks = st.num_blocks;
-    if(block_offset) *block_offset = st.block_offset;
-    if(stopped) *stopped = st.stopped;
-    return B200MIX_OK;
-}
+{ return d ? d->buffers.callback_state(buffer, num_blocks, block_offset, stopped) : B200MIX_ERR_INVALID; }
 
 int b200mix_buffer_data(b200mix_device *d, uint32_t buffer, uint32_t sample_type, uint32_t channels,
     uint32_t frames, const void *data, size_t bytes)
-{
-    if(!d) return B200MIX_ERR_INVALID;
-    static const size_t sz[] = {1, 2, 4, 4, 8, 1, 1};
-    if(buffer >= d->desc.max_buffers || sample_type > B200MIX_FMT_ALAW || channels < 1 || !data)
-    { d->error = "buffer_data: bad arguments"; return B200MIX_ERR_INVALID; }
-    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(int rc = cb_unregister(d, buffer, "buffer_data")) return rc;
-    const size_t need = size_t(frames)*channels*sz[sample_type];
-    if(bytes < need) { d->error = "buffer_data: short data"; return B200MIX_ERR_INVALID; }
-    BufferRec &h = d->h_buffers[buffer];
-    if(h.data && d->book.bufrefs[buffer])
-    { d->error = "buffer_data: the buffer is attached to an active voice (AL_INVALID_OPERATION)"; return B200MIX_ERR_INVALID; }
-    DevArray<char> &store = d->buf_store[buffer];
-    if(h.data)
-    {
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        store.reset();
-        h = BufferRec{};
-    }
-    // +16 bytes so vector/tail reads past the last frame stay inside the allocation
-    CUDA_TRY(d, store.alloc(need + 16));
-    CUDA_TRY(d, cudaMemcpyAsync(store.get(), data, need, cudaMemcpyHostToDevice, d->stream));
-    h.data = store.get(); h.frames = frames; h.type = sample_type; h.channels = channels;
-    CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec), cudaMemcpyHostToDevice,
-        d->stream));
-    return B200MIX_OK;
-}
+{ return set_buffer(d, &BufferTable::set_data, buffer, sample_type, channels, frames, data, bytes); }
 
 int b200mix_buffer_data_adpcm(b200mix_device *d, uint32_t buffer, uint32_t sample_type,
     uint32_t channels, uint32_t samples_per_block, uint32_t blocks, const void *data, size_t bytes)
@@ -782,31 +630,12 @@ int b200mix_buffer_data_adpcm(b200mix_device *d, uint32_t buffer, uint32_t sampl
     std::vector<int16_t> pcm(size_t(blocks)*samples_per_block*channels);
     if(ms) DecodeMSADPCM(static_cast<const uint8_t*>(data), channels, samples_per_block, blocks, pcm.data());
     else DecodeIMA4(static_cast<const uint8_t*>(data), channels, samples_per_block, blocks, pcm.data());
-    const int rc = b200mix_buffer_data(d, buffer, B200MIX_FMT_I16, channels, blocks*samples_per_block,
+    return b200mix_buffer_data(d, buffer, B200MIX_FMT_I16, channels, blocks*samples_per_block,
         pcm.data(), pcm.size()*sizeof(int16_t));
-    // the upload above reads pageable memory: make sure it is consumed before pcm goes away
-    if(rc == B200MIX_OK) CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-    return rc;
 }
 
 int b200mix_buffer_free(b200mix_device *d, uint32_t buffer)
-{
-    if(!d || buffer >= d->desc.max_buffers) return B200MIX_ERR_INVALID;
-    CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
-    if(int rc = cb_unregister(d, buffer, "buffer_free")) return rc;
-    BufferRec &h = d->h_buffers[buffer];
-    if(h.data && d->book.bufrefs[buffer])
-    { d->error = "buffer_free: the buffer is attached to an active voice; stop the voice first"; return B200MIX_ERR_INVALID; }
-    if(h.data)
-    {
-        CUDA_TRY(d, cudaStreamSynchronize(d->stream));
-        d->buf_store[buffer].reset();
-        h = BufferRec{};
-        CUDA_TRY(d, cudaMemcpyAsync(d->d_buffers + buffer, &h, sizeof(BufferRec),
-            cudaMemcpyHostToDevice, d->stream));
-    }
-    return B200MIX_OK;
-}
+{ return set_buffer(d, &BufferTable::free, buffer); }
 
 int b200mix_slot_disable(b200mix_device *d, uint32_t slot)
 {
@@ -1184,33 +1013,6 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
     const float *hrtf_coeffs, const float *dirs, const float *dry_gains, const float *send_gains,
     bool direct);
 
-// The voices of each callback buffer are the channels of one source: cb_reps[slot] = the first one
-// that mixes this update (-1: none), cb_members[slot] the others, which must agree with it on what
-// the planner reads.  One pass over the voices.
-static int cb_group(b200mix_device *d)
-{
-    std::vector<int32_t> &reps = d->cb_reps;
-    reps.assign(d->cbs.size(), -1);
-    d->cb_members.resize(d->cbs.size());
-    for(auto &m : d->cb_members) m.clear();
-    for(uint32_t v = 0;v < d->book.voice_hi;++v)
-    {
-        const b200mix_device::CbVoice &cv = d->cbv[v];
-        if(cv.slot < 0 || (cv.v.state != 1u && cv.v.state != 2u)) continue;
-        int32_t &r = reps[size_t(cv.slot)];
-        if(r < 0) { r = int32_t(v); continue; }
-        const cbplan::Voice &a = d->cbv[size_t(r)].v, &b = cv.v;
-        if(a.pos != b.pos || a.frac != b.frac || a.step != b.step || a.state != b.state
-            || a.have_buffer != b.have_buffer)
-        {
-            d->error = "voices_update: voices sharing a callback buffer disagree on step, position or state";
-            return B200MIX_ERR_INVALID;
-        }
-        d->cb_members[size_t(cv.slot)].push_back(v);
-    }
-    return B200MIX_OK;
-}
-
 int b200mix_voices_update(b200mix_device *d, uint32_t n, const b200mix_voice_params *params,
     const float *hrtf_coeffs, const float *dry_gains, const float *send_gains)
 {
@@ -1265,13 +1067,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         // with directions the delays are computed on the device
         if(!dirs && (p.hrtf_delay[0] >= B200MIX_HRTF_HISTORY || p.hrtf_delay[1] >= B200MIX_HRTF_HISTORY))
         { d->error = "voices_update: HRTF delay out of range"; return B200MIX_ERR_INVALID; }
-        // callback voice: plays a buffer made by b200mix_buffer_callback
-        const int32_t cbSlot = cb_slot_of(d, p.flags, p.buffer);
-        if(cbSlot >= 0 && (p.flags & B200MIX_VF_STATIC))
-        { d->error = "voices_update: a callback buffer is not static (IsCallback)"; return B200MIX_ERR_INVALID; }
-        if(cbSlot >= 0 && d->cbv[p.voice].slot != cbSlot && !(p.flags & B200MIX_VF_RESET))
-        { d->error = "voices_update: a voice starts a callback buffer with B200MIX_VF_RESET"; return B200MIX_ERR_INVALID; }
     }
+    if(int rc = d->buffers.check_voices(n, params)) return rc;
 
     if(direct)
         if(int rc = ensure_real_bus(d)) return rc;
@@ -1306,33 +1103,8 @@ static int voices_update_impl(b200mix_device *d, uint32_t n, const b200mix_voice
         d->book.set(p.voice, {!stopped, cost, (p.flags & B200MIX_VF_HRTF) != 0, p.send_slot,
             (p.flags & B200MIX_VF_STATIC) && !nobuf ? p.buffer : B200MIX_NO_SLOT, (p.flags & B200MIX_VF_RESET) != 0,
             direct});
-        if(!d->cbv.empty())
-        {
-            // the planner's mirror of the voice: what k_apply_updates does to its record
-            b200mix_device::CbVoice &cv = d->cbv[p.voice];
-            const int32_t slot = nobuf && !stopped ? cv.slot : cb_slot_of(d, p.flags, p.buffer);
-            if(slot != cv.slot)
-            {
-                d->cb_bound = d->cb_bound + (slot >= 0) - (cv.slot >= 0);
-                cv.slot = slot;
-            }
-            if(slot >= 0)
-            {
-                cbplan::Voice &m = cv.v;
-                if(p.flags & B200MIX_VF_RESET)
-                {
-                    m.pos = p.position; m.frac = p.position_frac; m.have_buffer = true;
-                    d->cbs[size_t(slot)].st = cbplan::State{};
-                }
-                if(p.flags & B200MIX_VF_STOPPING) m.state = 2u;
-                else if(p.flags & B200MIX_VF_PLAYING) m.state = 1u;
-                m.step = p.step;
-                if(nobuf) m.have_buffer = false;
-            }
-        }
+        d->buffers.apply_voice(p);
     }
-    if(d->cb_bound)
-        if(int rc = cb_group(d)) return rc;
     ApplyParams A = apply_params(d, d->stage.dev_of(upd));
     auto pack = [d](const float *src, size_t count) { return d->stage.pack(src, count); };
     if(dirs && dd.ir_size)
@@ -1397,7 +1169,7 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
         if(int rc = check_entry(d, "sources_update", p, false, hrtfMode)) return rc;
         // callback voices are planned from the steps b200mix_voices_update gives; this stage
         // computes them on the device, where the planner cannot see them
-        if(cb_slot_of(d, p.flags, p.buffer) >= 0)
+        if(d->buffers.cb_slot(p.flags, p.buffer) >= 0)
         { d->error = "sources_update: callback buffers play through b200mix_voices_update"; return B200MIX_ERR_UNSUPPORTED; }
         if(!mayFilter && source_may_filter(P, dd.num_sends)) mayFilter = true;
     }
@@ -1420,12 +1192,7 @@ int b200mix_sources_update(b200mix_device *d, uint32_t n, const b200mix_source_v
     {
         const b200mix_source_voice &p = voices[i];
         const bool act = !(p.flags & B200MIX_VF_STOPPED);
-        // the voice no longer plays a callback buffer
-        if(!d->cbv.empty() && d->cbv[p.voice].slot >= 0)
-        {
-            d->cbv[p.voice].slot = -1;
-            --d->cb_bound;
-        }
+        d->buffers.unbind(p.voice);           // it no longer plays a callback buffer
         // the step is not known here: the cost key takes the resampler's widest filter, and is
         // kept while the voice stays active
         const BsincTable *t = bsinc_for(d, p.resampler);
@@ -1541,7 +1308,7 @@ int b200mix_voice_queue(b200mix_device *d, uint32_t voice, uint32_t count, const
     Q.voice = voice; Q.count = count; Q.loop = loop_index;
     for(uint32_t i = 0;i < count;++i)
     {
-        if(buffers[i] >= dd.max_buffers || !d->h_buffers[buffers[i]].data || d->h_buffers[buffers[i]].pad)
+        if(!d->buffers.queueable(buffers[i]))
         { d->error = "voice_queue: buffer id without data"; return B200MIX_ERR_INVALID; }
         Q.items[i] = buffers[i];
     }
@@ -1650,88 +1417,6 @@ static int run_bus_mix(b200mix_device *d, const SendMixParams &M, uint32_t num_e
 static inline void stage_mark(b200mix_device *d, int i)
 { if(d->profile_level >= 2) cudaEventRecord(d->ev_stage[i], d->stream); }
 
-// The callback buffers' part of an update (callback_plan.hpp).  First every callback buffer's
-// callbacks run on this thread; then, straight into the pinned arena, each buffer's plan record and
-// the blocks it has stored (ADPCM decoded to int16) are packed, its storage is compacted as the
-// reference does after the mix, and its voices' mirror advances; table and samples go to the GPU
-// with one copy on the mixer stream.  *plan stays null when no callback voice mixes this update.
-static int cb_plan_update(b200mix_device *d, uint32_t frames, const BufferRec *&plan)
-{
-    plan = nullptr;
-    if(int rc = cb_group(d)) { d->error = "render: " + d->error; return rc; }
-    const std::vector<int32_t> &reps = d->cb_reps;
-    bool any = false;
-    for(int32_t r : reps) any = any || r >= 0;
-    if(!any) return B200MIX_OK;
-    d->cb_work.resize(d->cbs.size());
-    // 1. the callbacks.  Registration guarantees the reference's storage size, which no request of
-    //    its chunk loop passes: plan_loads cannot stop half way through the buffers.
-    size_t size = align16(d->cbs.size()*sizeof(BufferRec));
-    for(size_t s = 0;s < d->cbs.size();++s)
-    {
-        if(reps[s] < 0) continue;
-        b200mix_device::CbBuf &c = d->cbs[s];
-        b200mix_device::CbWork &w = d->cb_work[s];
-        const b200mix_callback_buffer &cb = c.cb;
-        auto request = [&cb](uint64_t offset, uint32_t bytes) -> int64_t {
-            return cb.callback(cb.userptr, static_cast<char*>(cb.storage) + offset, int(bytes));
-        };
-        w.start = c.st;
-        if(!cbplan::plan_loads(c.st, cb.samples_per_block, cb.bytes_per_block, d->cbv[size_t(reps[s])].v,
-            frames, cb.storage_bytes, request, w.loads))
-        { d->error = "render: a callback request passes the callback buffer's storage"; return B200MIX_ERR_INVALID; }
-        // [pad | the stored blocks as the kernel reads them | pad], a pad holding one frame and
-        // 16 bytes: a load held at the last stored sample may address the frame before the first
-        // (none stored) or the first (empty span); the bulk copies round their runs up to 16 bytes
-        const size_t pad = align16(c.frame_bytes) + 16u;
-        w.bytes = w.loads.chunks ? size_t(c.st.num_blocks)*cb.samples_per_block*c.frame_bytes : 0u;
-        w.region = size + pad;
-        size = w.region + align16(w.bytes) + pad;
-    }
-    // 2. the arena (two alternate: the other one's copy may still be in flight)
-    UploadArena &U = d->cb_arena[d->cb_idx];
-    CUDA_TRY(d, U.wait());
-    CUDA_TRY(d, U.reserve(size, size*2, size*2, size*2, d->stream));
-    U.begin();
-    uint8_t *arena = U.host_part<uint8_t>(size);
-    const uintptr_t devArena = reinterpret_cast<uintptr_t>(U.dev_of(arena));
-    // 3. pack, then what the reference does after the mix
-    std::memset(arena, 0, size);
-    for(size_t s = 0;s < d->cbs.size();++s)
-    {
-        if(reps[s] < 0) continue;
-        b200mix_device::CbBuf &c = d->cbs[s];
-        const b200mix_device::CbWork &w = d->cb_work[s];
-        const b200mix_callback_buffer &cb = c.cb;
-        cbplan::Voice &vm = d->cbv[size_t(reps[s])].v;
-        const cbplan::Span span = cbplan::span_of(w.start, vm, cb.samples_per_block, c.st);
-        BufferRec rec = d->h_buffers[c.buffer];
-        rec.data = reinterpret_cast<const void*>(devArena
-            + uintptr_t(int64_t(w.region) + span.base*int64_t(c.frame_bytes)));
-        rec.frames = w.loads.chunks ? span.frames : 0u;
-        std::memcpy(arena + s*sizeof(BufferRec), &rec, sizeof(rec));
-        uint8_t *dst = arena + w.region;
-        const uint8_t *src = static_cast<const uint8_t*>(cb.storage);
-        if(!w.bytes) {}
-        else if(cb.sample_type == B200MIX_FMT_IMA4)
-            DecodeIMA4(src, cb.channels, cb.samples_per_block, c.st.num_blocks, reinterpret_cast<int16_t*>(dst));
-        else if(cb.sample_type == B200MIX_FMT_MSADPCM)
-            DecodeMSADPCM(src, cb.channels, cb.samples_per_block, c.st.num_blocks, reinterpret_cast<int16_t*>(dst));
-        else
-            std::memcpy(dst, src, w.bytes);
-        const cbplan::After after = cbplan::finish_update(c.st, cb.samples_per_block, cb.bytes_per_block,
-            vm, frames);
-        if(after.consumed_bytes)
-            std::memmove(cb.storage, static_cast<char*>(cb.storage) + after.consumed_bytes, after.kept_bytes);
-        // the source's other channel voices move with it
-        for(uint32_t v : d->cb_members[s]) d->cbv[v].v = vm;
-    }
-    CUDA_TRY(d, U.ship(d->stream));
-    d->cb_idx ^= 1;
-    plan = reinterpret_cast<const BufferRec*>(devArena);
-    return B200MIX_OK;
-}
-
 // Phase A of an update: clear the mix buffers, mix every voice, reduce the partial rows and
 // finish the aux sends -> the slots' Wet buffers are complete (alc/alu.cpp:2196-2206).
 static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results, bool force_sends)
@@ -1743,8 +1428,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     CUDA_TRY(d, cudaSetDevice(d->cuda_dev));
     // callback buffers: their callbacks run here, before anything of the update is launched
     const BufferRec *cbplan = nullptr;
-    if(d->cb_bound)
-        if(int rc = cb_plan_update(d, frames, cbplan)) return rc;
+    if(int rc = d->buffers.plan(frames, cbplan)) return rc;
 
     VoiceBook &B = d->book;
     const VoiceBook::Rebuilt re = B.refresh(d->d_filt != nullptr, d->mix_cdr == 0 && d->d_dry_entries,
@@ -1792,7 +1476,7 @@ static int render_phase_a(b200mix_device *d, uint32_t frames, bool want_results,
     const uint32_t blocks = std::max(1u, std::min(maxBlocks, (numOrder + kMixGroups - 1)/kMixGroups));
 
     MixParams P{};
-    P.voices = d->d_voices; P.buffers = d->d_buffers;
+    P.voices = d->d_voices; P.buffers = d->buffers.device();
     P.hrtf_tgt = d->d_hrtf_tgt; P.hrtf_old = d->d_hrtf_old;
     P.dry_cur = d->d_dry_cur; P.dry_tgt = d->d_dry_tgt;
     P.partial = d->d_partial;
