@@ -9,6 +9,7 @@
 #include <cstddef>
 #include <cstring>
 #include <utility>
+#include <vector>
 
 #include <cuda_runtime.h>
 
@@ -77,6 +78,17 @@ cudaError_t regrow(DevArray<T> &a, size_t count, cudaStream_t stream)
 {
     const cudaError_t e = cudaStreamSynchronize(stream);
     return e != cudaSuccess ? e : a.alloc(count);
+}
+
+// Copies a host vector to the front of a device array, then synchronises the stream: the vector
+// may be rebuilt (or go away) before an asynchronous copy would have read it.
+template<typename T>
+cudaError_t upload(DevArray<T> &dst, const std::vector<T> &src, cudaStream_t stream)
+{
+    if(!src.empty())
+        if(const cudaError_t e = cudaMemcpyAsync(dst.get(), src.data(), src.size()*sizeof(T), cudaMemcpyHostToDevice,
+            stream)) return e;
+    return cudaStreamSynchronize(stream);
 }
 
 // A pinned block and a device block that one call packs its inputs into (16-byte aligned parts)
