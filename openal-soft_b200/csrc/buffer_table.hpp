@@ -12,13 +12,11 @@
 #include "../../include/b200mix.h"
 #include "mixer_kernels.cuh"
 #include "device_memory.hpp"
+#include "launch.hpp"
 #include "callback_plan.hpp"
 #include "adpcm.hpp"
 
 namespace b200mix {
-
-// Every call below returns a B200MIX_* code and, when it fails, sets the device's error string.
-#define BUF_TRY(expr) do { const cudaError_t e_ = (expr); if(e_ != cudaSuccess) return fail(#expr, e_); } while(0)
 
 class BufferTable {
 public:
@@ -28,8 +26,8 @@ public:
         n_ = max_buffers; s_ = stream; err_ = &err;
         bufs_.resize(std::max(max_buffers, 1u));
         voices_.assign(max_voices, CbVoice{});
-        BUF_TRY(d_buffers_.alloc(bufs_.size(), s_));
-        BUF_TRY(zero_.alloc(kCbPad, s_));
+        CUDA_TRY(*err_, d_buffers_.alloc(bufs_.size(), s_));
+        CUDA_TRY(*err_, zero_.alloc(kCbPad, s_));
         return B200MIX_OK;
     }
     const BufferRec *device() const { return d_buffers_; }
@@ -41,13 +39,13 @@ public:
         size_t bytes, const std::vector<uint32_t> &bufrefs)
     {
         if(buffer >= n_ || sample_type > B200MIX_FMT_ALAW || channels < 1 || !data)
-            return refuse("buffer_data: bad arguments");
+            return refuse(*err_, "buffer_data: bad arguments");
         const size_t need = size_t(frames)*channels*kSampleBytes[sample_type];
-        if(bytes < need) return refuse("buffer_data: short data");
+        if(bytes < need) return refuse(*err_, "buffer_data: short data");
         if(int rc = releasable(buffer, bufrefs, "buffer_data", kHeld)) return rc;
         Buf next;
-        BUF_TRY(next.store.alloc(need + 16));   // +16 bytes: vector/tail reads past the last frame stay inside
-        BUF_TRY(cudaMemcpyAsync(next.store.get(), data, need, cudaMemcpyHostToDevice, s_));
+        CUDA_TRY(*err_, next.store.alloc(need + 16));   // +16 bytes: vector/tail reads past the last frame stay inside
+        CUDA_TRY(*err_, cudaMemcpyAsync(next.store.get(), data, need, cudaMemcpyHostToDevice, s_));
         next.rec = BufferRec{next.store.get(), frames, sample_type, channels, 0u};
         return commit(buffer, std::move(next));
     }
@@ -58,13 +56,13 @@ public:
         if(buffer >= n_ || !cb || cb->struct_size != sizeof(b200mix_callback_buffer) || !cb->callback
             || cb->sample_type > B200MIX_FMT_MSADPCM || cb->channels < 1 || !cb->storage
             || cb->samples_per_block < 1 || cb->bytes_per_block < 1)
-            return refuse("buffer_callback: bad arguments");
+            return refuse(*err_, "buffer_callback: bad arguments");
         const bool adpcm = cb->sample_type >= B200MIX_FMT_IMA4;
         const bool ms = cb->sample_type == B200MIX_FMT_MSADPCM;
         if(adpcm ? (cb->channels > 2 || !AdpcmBlockValid(ms, cb->samples_per_block)
                     || cb->bytes_per_block != AdpcmBlockBytes(ms, cb->channels, cb->samples_per_block))
                  : (cb->samples_per_block != 1u || cb->bytes_per_block != cb->channels*kSampleBytes[cb->sample_type]))
-            return refuse("buffer_callback: block size does not match the format");
+            return refuse(*err_, "buffer_callback: block size does not match the format");
         if(cb->channels > 16u)
         { *err_ = "buffer_callback: more than 16 channels"; return B200MIX_ERR_UNSUPPORTED; }
         // PrepareCallback's size (al/buffer.cpp:468-473): MixerLineSize*MaxPitch + MaxResamplerEdge
@@ -72,9 +70,9 @@ public:
         // callbacks of an update never stop half way.
         const uint64_t lineBlocks = ((1024u + 256u)*10u + 24u + cb->samples_per_block - 1u) / cb->samples_per_block;
         if(cb->storage_bytes < lineBlocks*cb->bytes_per_block)
-            return refuse("buffer_callback: storage smaller than the reference's callback storage");
+            return refuse(*err_, "buffer_callback: storage smaller than the reference's callback storage");
         if(uint64_t(cb->num_blocks)*cb->bytes_per_block > cb->storage_bytes || cb->stopped > 1u)
-            return refuse("buffer_callback: state outside the storage");
+            return refuse(*err_, "buffer_callback: state outside the storage");
         int32_t s = bufs_[buffer].slot;    // a registered buffer keeps its slot, and its voices play on
         if(int rc = s < 0 ? releasable(buffer, bufrefs, "buffer_callback", kHeld) : B200MIX_OK) return rc;
         if(s < 0) s = int32_t(std::find(slots_.begin(), slots_.end(), B200MIX_NO_BUFFER) - slots_.begin());
@@ -96,7 +94,7 @@ public:
     // The state of a callback buffer after the last update (b200mix_buffer_callback_state).
     int callback_state(uint32_t buffer, uint32_t *num_blocks, uint32_t *block_offset, uint32_t *stopped)
     {
-        if(buffer >= n_ || bufs_[buffer].slot < 0) return refuse("buffer_callback_state: not a callback buffer");
+        if(buffer >= n_ || bufs_[buffer].slot < 0) return refuse(*err_, "buffer_callback_state: not a callback buffer");
         const cbplan::State &st = bufs_[buffer].st;
         if(num_blocks) *num_blocks = st.num_blocks;
         if(block_offset) *block_offset = st.block_offset;
@@ -130,15 +128,15 @@ public:
             const int32_t s = cb_slot(p.flags, p.buffer);
             const CbVoice cur = p.voice < next_.size() ? next_[p.voice] : CbVoice{};
             if(s >= 0 && (p.flags & B200MIX_VF_STATIC))
-                return refuse("voices_update: a callback buffer is not static (IsCallback)");
+                return refuse(*err_, "voices_update: a callback buffer is not static (IsCallback)");
             if(s >= 0 && cur.slot != s && !(p.flags & B200MIX_VF_RESET))
-                return refuse("voices_update: a voice starts a callback buffer with B200MIX_VF_RESET");
+                return refuse(*err_, "voices_update: a voice starts a callback buffer with B200MIX_VF_RESET");
             const CbVoice nx = next_voice(cur, p);
             if(nx.slot >= 0 && p.voice >= next_.size()) next_.resize(p.voice + 1u);
             if(p.voice < next_.size()) next_[p.voice] = nx;
         }
         return group(next_, uint32_t(next_.size())) ? B200MIX_OK
-            : refuse("voices_update: voices sharing a callback buffer disagree on step, position or state");
+            : refuse(*err_, "voices_update: voices sharing a callback buffer disagree on step, position or state");
     }
 
     // What a checked entry does to the mirror (what k_apply_updates does to the voice's record).
@@ -183,7 +181,7 @@ public:
             w.start = c.st;
             if(!cbplan::plan_loads(c.st, cb.samples_per_block, cb.bytes_per_block, voices_[size_t(reps_[s])].v,
                 frames, cb.storage_bytes, request, w.loads))
-                return refuse("render: a callback request passes the callback buffer's storage");
+                return refuse(*err_, "render: a callback request passes the callback buffer's storage");
             // [pad | the stored blocks as the kernel reads them | pad], a pad holding one frame and
             // 16 bytes: a load held at the last stored sample may address the frame before the first
             // (none stored) or the first (empty span); the bulk copies round their runs up to 16 bytes
@@ -194,8 +192,8 @@ public:
         }
         // 2. the arena (two alternate: the other one's copy may still be in flight)
         UploadArena &U = arena_[idx_];
-        BUF_TRY(U.wait());
-        BUF_TRY(U.reserve(size, size*2, size*2, size*2, s_));
+        CUDA_TRY(*err_, U.wait());
+        CUDA_TRY(*err_, U.reserve(size, size*2, size*2, size*2, s_));
         U.begin();
         uint8_t *arena = U.host_part<uint8_t>(size);
         const uintptr_t devArena = reinterpret_cast<uintptr_t>(U.dev_of(arena));
@@ -230,7 +228,7 @@ public:
             // the source's other channel voices move with it
             for(uint32_t v : members_[s]) voices_[v].v = vm;
         }
-        BUF_TRY(U.ship(s_));
+        CUDA_TRY(*err_, U.ship(s_));
         idx_ ^= 1;
         plan = reinterpret_cast<const BufferRec*>(devArena);
         return B200MIX_OK;
@@ -250,9 +248,6 @@ private:
     struct CbVoice { int32_t slot{-1}; cbplan::Voice v{}; };
     struct CbWork { cbplan::State start; cbplan::Loads loads; size_t region{0}, bytes{0}; };
 
-    int refuse(const std::string &why) { *err_ = why; return B200MIX_ERR_INVALID; }
-    int fail(const char *what, cudaError_t e) { *err_ = std::string(what) + ": " + cudaGetErrorString(e); return B200MIX_ERR_CUDA; }
-
     // No callback buffer is registered or played: the mirror has nothing to follow.
     bool idle() const { return !bound_ && std::all_of(slots_.begin(), slots_.end(), [](uint32_t b) { return b == B200MIX_NO_BUFFER; }); }
 
@@ -262,16 +257,16 @@ private:
         const Buf &b = bufs_[buffer];
         if(b.slot >= 0 && std::any_of(voices_.begin(), voices_.begin() + hi_, [&b](const CbVoice &cv)
             { return cv.slot == b.slot && (cv.v.state == 1u || cv.v.state == 2u); }))
-            return refuse(std::string(what) + ": the callback buffer is played by a voice; stop it first");
-        return b.rec.data && bufrefs[buffer] ? refuse(std::string(what) + ": " + held) : B200MIX_OK;
+            return refuse(*err_, std::string(what) + ": the callback buffer is played by a voice; stop it first");
+        return b.rec.data && bufrefs[buffer] ? refuse(*err_, std::string(what) + ": " + held) : B200MIX_OK;
     }
 
     // Once the stream is idle (queued kernels may still read what is replaced, and `next`'s copies
     // have landed), `next` replaces the buffer; a registration that ends unbinds its voices.
     int commit(uint32_t buffer, Buf &&next)
     {
-        BUF_TRY(cudaMemcpyAsync(d_buffers_ + buffer, &next.rec, sizeof(BufferRec), cudaMemcpyHostToDevice, s_));
-        BUF_TRY(cudaStreamSynchronize(s_));
+        CUDA_TRY(*err_, cudaMemcpyAsync(d_buffers_ + buffer, &next.rec, sizeof(BufferRec), cudaMemcpyHostToDevice, s_));
+        CUDA_TRY(*err_, cudaStreamSynchronize(s_));
         Buf &b = bufs_[buffer];
         if(b.slot >= 0 && b.slot != next.slot)
         {
@@ -332,6 +327,5 @@ private:
     std::vector<CbWork> work_;           // per slot, for the update being planned
 };
 
-#undef BUF_TRY
 
 } // namespace b200mix

@@ -18,9 +18,6 @@ namespace b200mix {
 
 static_assert(kPostMaxDry == B200MIX_MAX_DRY_CHANNELS, "k_post_hrtf_reduce: one thread per dry channel");
 
-// Every call below returns a B200MIX_* code and, when it fails, sets the device's error string.
-#define OUT_TRY(expr) do { const cudaError_t e_ = (expr); if(e_ != cudaSuccess) return fail(#expr, e_); } while(0)
-
 class OutputStage {
 public:
     // What every update may use: the HRTF accumulator carry, the decoders' band-split scratch, the
@@ -30,13 +27,13 @@ public:
     {
         dd_ = dd; s_ = stream; err_ = &err;
         const size_t temp = size_t(std::max(dd.dry_channels, 1u))*kLine;
-        for(DevArray<float> &c : carry_) OUT_TRY(c.alloc(2*kHrirLen, s_));
-        OUT_TRY(temp_.alloc(temp, s_));
-        OUT_TRY(temp2_.alloc(temp, s_));
-        OUT_TRY(d_outbuf_.alloc(size_t(kLine)*64*4));
-        OUT_TRY(h_outbuf_.alloc(size_t(kLine)*64*4));
+        for(DevArray<float> &c : carry_) CUDA_TRY(*err_, c.alloc(2*kHrirLen, s_));
+        CUDA_TRY(*err_, temp_.alloc(temp, s_));
+        CUDA_TRY(*err_, temp2_.alloc(temp, s_));
+        CUDA_TRY(*err_, d_outbuf_.alloc(size_t(kLine)*64*4));
+        CUDA_TRY(*err_, h_outbuf_.alloc(size_t(kLine)*64*4));
         if(dd.post_process == B200MIX_POST_UHJ || dd.post_process == B200MIX_POST_TSME)
-            OUT_TRY(uhj_.state.alloc(64, s_));
+            CUDA_TRY(*err_, uhj_.state.alloc(64, s_));
         return B200MIX_OK;
     }
 
@@ -63,13 +60,13 @@ public:
     {
         if(channels != dd_.dry_channels || ir > B200MIX_HRIR_LENGTH || !coeffs || !hf_scale || !splitter
             || dd_.post_process != B200MIX_POST_HRTF)
-            return refuse("set_hrtf_decoder: bad arguments");
+            return refuse(*err_, "set_hrtf_decoder: bad arguments");
         HrtfDecoder next{channels, ir};
         std::vector<float> st(size_t(channels)*4, 0.0f);
         for(uint32_t c = 0;c < channels;++c) st[c*4] = splitter[c];
-        OUT_TRY(fill(next.coef, reinterpret_cast<const float2*>(coeffs), size_t(channels)*ir));
-        OUT_TRY(fill(next.hfscale, hf_scale, channels));
-        OUT_TRY(fill(next.state, st.data(), st.size()));
+        CUDA_TRY(*err_, fill(next.coef, reinterpret_cast<const float2*>(coeffs), size_t(channels)*ir));
+        CUDA_TRY(*err_, fill(next.hfscale, hf_scale, channels));
+        CUDA_TRY(*err_, fill(next.state, st.data(), st.size()));
         return commit(hrtf_, next);
     }
 
@@ -77,14 +74,14 @@ public:
     int set_ambi_decoder(uint32_t in_channels, const float *gains_hf, const float *gains_lf, float xover_coeff)
     {
         if(in_channels != dd_.dry_channels || !gains_hf || dd_.post_process != B200MIX_POST_AMBIDEC)
-            return refuse("set_ambi_decoder: bad arguments");
+            return refuse(*err_, "set_ambi_decoder: bad arguments");
         const size_t n = size_t(in_channels)*dd_.real_channels;
         AmbiDecoder next{in_channels, gains_lf != nullptr};
         std::vector<float> st(size_t(in_channels)*4, 0.0f);
         for(uint32_t c = 0;c < in_channels;++c) st[c*4] = xover_coeff;
-        OUT_TRY(fill(next.hf, gains_hf, n));
-        if(gains_lf) OUT_TRY(fill(next.lf, gains_lf, n));
-        OUT_TRY(fill(next.state, st.data(), st.size()));
+        CUDA_TRY(*err_, fill(next.hf, gains_hf, n));
+        if(gains_lf) CUDA_TRY(*err_, fill(next.lf, gains_lf, n));
+        CUDA_TRY(*err_, fill(next.state, st.data(), st.size()));
         return commit(ambi_, next);
     }
 
@@ -94,13 +91,13 @@ public:
     {
         if((dd_.post_process != B200MIX_POST_UHJ && dd_.post_process != B200MIX_POST_TSME) || dd_.dry_channels < 3
             || (filter_length != 0 && filter_length != 256 && filter_length != 512))
-            return refuse("set_uhj_encoder: needs a UHJ device and a length of 0, 256 or 512");
+            return refuse(*err_, "set_uhj_encoder: needs a UHJ device and a length of 0, 256 or 512");
         UhjEncoder next{filter_length};
-        OUT_TRY(next.state.alloc(64, s_));
+        CUDA_TRY(*err_, next.state.alloc(64, s_));
         std::vector<float> coef(256, 0.0f);
         if(filter_length)
         {
-            OUT_TRY(next.fir_state.alloc(kUhjFirStateFloats, s_));
+            CUDA_TRY(*err_, next.fir_state.alloc(kUhjFirStateFloats, s_));
             // SegmentedFilter's desired response (core/allpass_conv.hpp:56-75): Blackman-Nuttall
             // windowed 2/(pi k) at the odd taps
             const uint32_t half = filter_length/2u;
@@ -113,7 +110,7 @@ public:
                     - 0.0106411*std::cos(3.0*w);
                 coef[i] = float(window * 2.0 / (pi * double(k)));
             }
-            OUT_TRY(fill(next.fir_coef, coef.data(), coef.size()));
+            CUDA_TRY(*err_, fill(next.fir_coef, coef.data(), coef.size()));
         }
         if(int rc = commit(uhj_, next)) return rc;
         if(delay) *delay = filter_length ? filter_length/2u + 128u : 1u;
@@ -128,9 +125,9 @@ public:
         {
             if(dd_.post_process != B200MIX_POST_AMBIDEC || center_channel >= dd_.real_channels || !stereo()
                 || center_channel == dd_.real_left || center_channel == dd_.real_right || dd_.real_channels > 32u)
-                return refuse("set_front_stabilizer: needs an ambisonic-decode device with left, right and centre outputs");
-            OUT_TRY(next.state.alloc(4 + 32, s_));
-            OUT_TRY(cudaFuncSetAttribute(k_post_stabilizer, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                return refuse(*err_, "set_front_stabilizer: needs an ambisonic-decode device with left, right and centre outputs");
+            CUDA_TRY(*err_, next.state.alloc(4 + 32, s_));
+            CUDA_TRY(*err_, cudaFuncSetAttribute(k_post_stabilizer, cudaFuncAttributeMaxDynamicSharedMemorySize,
                 int(size_t(2u + dd_.real_channels)*kLine*sizeof(float))));
         }
         return commit(stab_, next);
@@ -140,7 +137,7 @@ public:
     int set_bs2b(uint32_t level)
     {
         if(level > 6 || dd_.post_process != B200MIX_POST_AMBIDEC || !stereo())
-            return refuse("set_bs2b: needs a stereo ambisonic-decode device and a level of 0..6");
+            return refuse(*err_, "set_bs2b: needs a stereo ambisonic-decode device and a level of 0..6");
         Bs2b next{level};
         float h[9] = {};
         if(level)
@@ -161,8 +158,8 @@ public:
             h[4+1] = x; h[4+0] = G_lo * (1.0f - x) * g;
             x = std::exp(-pi*2.0f*Fc_hi/float(dd_.sample_rate));
             h[4+4] = x; h[4+2] = (1.0f - G_hi * (1.0f - x)) * g; h[4+3] = -x * g;
-            OUT_TRY(fill(next.buf, h, 9));
-            OUT_TRY(next.direct.alloc(2*kLine, s_));
+            CUDA_TRY(*err_, fill(next.buf, h, 9));
+            CUDA_TRY(*err_, next.direct.alloc(2*kLine, s_));
         }
         return commit(bs2b_, next);
     }
@@ -171,7 +168,7 @@ public:
     // expressions, by the host's libm, so the derived constants are the reference's bit for bit.
     int set_limiter(const b200mix_limiter_desc *p, uint32_t *look_ahead)
     {
-        if(p && p->struct_size != sizeof(*p)) return refuse("set_limiter: struct_size");
+        if(p && p->struct_size != sizeof(*p)) return refuse(*err_, "set_limiter: struct_size");
         Limiter next;
         LimiterDev h{};
         if(p)
@@ -197,8 +194,8 @@ public:
             h.gain_estimate = h.threshold * -0.5f * h.slope;
             h.adapt_coeff = std::exp(-1.0f / (2.0f * rate));
             for(float &v : h.hold_hist) v = -INFINITY;
-            OUT_TRY(fill(next.lim, &h, 1));
-            OUT_TRY(next.delay.alloc(size_t(std::max(dd_.real_channels, 1u))*kLine, s_));
+            CUDA_TRY(*err_, fill(next.lim, &h, 1));
+            CUDA_TRY(*err_, next.delay.alloc(size_t(std::max(dd_.real_channels, 1u))*kLine, s_));
         }
         if(int rc = commit(limiter_, next)) return rc;
         if(look_ahead) *look_ahead = h.look_ahead;
@@ -213,15 +210,15 @@ public:
         std::vector<float> hg(dd_.real_channels, 1.0f);
         if(channels)
         {
-            if(channels > dd_.real_channels || !delays || !gains) return refuse("set_distance_comp: bad arguments");
+            if(channels > dd_.real_channels || !delays || !gains) return refuse(*err_, "set_distance_comp: bad arguments");
             for(uint32_t c = 0;c < channels;++c)
             {
-                if(delays[c] >= kLine) return refuse("set_distance_comp: delay >= 1024");
+                if(delays[c] >= kLine) return refuse(*err_, "set_distance_comp: delay >= 1024");
                 hd[c] = delays[c]; hg[c] = gains[c];
             }
-            OUT_TRY(fill(next.delay, hd.data(), hd.size()));
-            OUT_TRY(fill(next.gain, hg.data(), hg.size()));
-            OUT_TRY(next.buf.alloc(size_t(dd_.real_channels)*kLine, s_));
+            CUDA_TRY(*err_, fill(next.delay, hd.data(), hd.size()));
+            CUDA_TRY(*err_, fill(next.gain, hg.data(), hg.size()));
+            CUDA_TRY(*err_, next.buf.alloc(size_t(dd_.real_channels)*kLine, s_));
         }
         return commit(dc_, next);
     }
@@ -243,11 +240,11 @@ public:
                 .cd = dd_.dry_channels, .dec_ir = hrtf_.ir, .real_left = dd_.real_left, .real_right = dd_.real_right,
                 .dry_active = dry_active};
             if(dry_active)
-                OUT_TRY(launch_ex(s_, launches, false, k_post_hrtf_split, dim3(dd_.dry_channels), dim3(32), 0, Q));
+                CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_hrtf_split, dim3(dd_.dry_channels), dim3(32), 0, Q));
             Q.overwrite = overwrites_real() && !direct ? 1u : 0u;
             // straight behind the HRIR FIR (no kernel of the dry bus, sends, effects or band split in
             // between), it is scheduled under the FIR's last CTAs
-            OUT_TRY(launch_ex(s_, launches, launches == fir_done, k_post_hrtf_reduce,
+            CUDA_TRY(*err_, launch_ex(s_, launches, launches == fir_done, k_post_hrtf_reduce,
                 dim3((frames + kHrirLen + kPostTile - 1)/kPostTile, 2), dim3(1024), 0, Q));
             carry_idx_ ^= 1;
             break;
@@ -263,12 +260,12 @@ public:
                 for(uint32_t k = 0;k < 2;++k)
                 {
                     float *ch = real + size_t(k ? dd_.real_right : dd_.real_left)*kLine;
-                    OUT_TRY(cudaMemcpyAsync(bs2b_.direct + k*kLine, ch, frames*sizeof(float),
+                    CUDA_TRY(*err_, cudaMemcpyAsync(bs2b_.direct + k*kLine, ch, frames*sizeof(float),
                         cudaMemcpyDeviceToDevice, s_));
-                    OUT_TRY(cudaMemsetAsync(ch, 0, frames*sizeof(float), s_));
+                    CUDA_TRY(*err_, cudaMemsetAsync(ch, 0, frames*sizeof(float), s_));
                 }
-            if(ambi_.dual) OUT_TRY(launch_ex(s_, launches, false, k_post_ambi_split, dim3(1), dim3(32), 0, Q));
-            OUT_TRY(launch_ex(s_, launches, false, k_post_ambi_mix, dim3((dd_.real_channels*frames + 127)/128),
+            if(ambi_.dual) CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_ambi_split, dim3(1), dim3(32), 0, Q));
+            CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_ambi_mix, dim3((dd_.real_channels*frames + 127)/128),
                 dim3(128), 0, Q));
             // with both installed, the stabilizer runs and BS2B does not (a device with a stabilizer
             // takes no direct-channel voices)
@@ -280,14 +277,14 @@ public:
                     .cidx = stab_.center, .coeff = stab_.coeff,
                     .mid_lf = std::cos(1.0f/3.0f * halfPi), .mid_hf = std::cos(1.0f/4.0f * halfPi),
                     .center_lf = std::sin(1.0f/3.0f * halfPi), .center_hf = std::sin(1.0f/4.0f * halfPi)};
-                OUT_TRY(launch_ex(s_, launches, false, k_post_stabilizer, dim3(1), dim3(32u*dd_.real_channels),
+                CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_stabilizer, dim3(1), dim3(32u*dd_.real_channels),
                     size_t(2u + dd_.real_channels)*kLine*sizeof(float), S));
             }
             else if(bs2b_.level)
             {
                 const Bs2bParams B{real, bs2b_.buf, bs2b_.buf + 4, frames, dd_.real_left, dd_.real_right,
                     bs2bDirect ? bs2b_.direct.get() : nullptr};
-                OUT_TRY(launch_ex(s_, launches, false, k_post_bs2b, dim3(1), dim3(128), 0, B));
+                CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_bs2b, dim3(1), dim3(128), 0, B));
             }
             break;
         }
@@ -295,10 +292,10 @@ public:
         {
             const MatrixEncSpec spec = dd_.post_process == B200MIX_POST_TSME ? kTsmeEncSpec : kUhjEncSpec;
             if(uhj_.fir)
-                OUT_TRY(launch_ex(s_, launches, false, k_post_uhj_fir, dim3(1), dim3(1024), 0, PostUhjFirParams{dry,
+                CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_uhj_fir, dim3(1), dim3(1024), 0, PostUhjFirParams{dry,
                     real, uhj_.fir_state, uhj_.fir_coef, frames, dd_.real_left, dd_.real_right, uhj_.fir, spec}));
             else
-                OUT_TRY(launch_ex(s_, launches, false, k_post_uhj, dim3(1), dim3(1024), 0, PostUhjParams{dry, real,
+                CUDA_TRY(*err_, launch_ex(s_, launches, false, k_post_uhj, dim3(1), dim3(1024), 0, PostUhjParams{dry, real,
                     uhj_.state, nullptr /* scratch: k_post_uhj reads none */, frames, dd_.real_left, dd_.real_right, spec}));
             break;
         }
@@ -311,10 +308,10 @@ public:
     int finish(float *real, uint32_t frames, uint64_t &launches)
     {
         if(limiter_.lim)
-            OUT_TRY(launch_ex(s_, launches, false, k_limiter, dim3(1), dim3(1024), 0,
+            CUDA_TRY(*err_, launch_ex(s_, launches, false, k_limiter, dim3(1), dim3(1024), 0,
                 LimiterParams{limiter_.lim, real, limiter_.delay, frames}));
         if(dc_.delay)
-            OUT_TRY(launch_ex(s_, launches, false, k_distance_comp, dim3(dd_.real_channels), dim3(1024), 0,
+            CUDA_TRY(*err_, launch_ex(s_, launches, false, k_distance_comp, dim3(dd_.real_channels), dim3(1024), 0,
                 DistCompParams{real, dc_.buf, dc_.delay, dc_.gain, frames}));
         return B200MIX_OK;
     }
@@ -327,9 +324,9 @@ public:
         const OutputParams Q{.real = real, .out = d_outbuf_, .frames = frames, .channels = dd_.real_channels,
             .frame_step = frame_step, .out_type = out_type, .seed = seed, .dither_depth = dither_depth};
         const uint32_t total = frames*frame_step;
-        OUT_TRY(launch_ex(s_, launches, false, k_output_write, dim3((total + 255)/256), dim3(256), 0, Q));
+        CUDA_TRY(*err_, launch_ex(s_, launches, false, k_output_write, dim3((total + 255)/256), dim3(256), 0, Q));
         out_bytes_ = size_t(total)*sz[out_type];
-        OUT_TRY(cudaMemcpyAsync(h_outbuf_, d_outbuf_, out_bytes_, cudaMemcpyDeviceToHost, s_));
+        CUDA_TRY(*err_, cudaMemcpyAsync(h_outbuf_, d_outbuf_, out_bytes_, cudaMemcpyDeviceToHost, s_));
         return B200MIX_OK;
     }
 
@@ -350,9 +347,6 @@ private:
 
     bool stereo() const
     { return dd_.real_left != dd_.real_right && dd_.real_left < dd_.real_channels && dd_.real_right < dd_.real_channels; }
-    int refuse(const char *why) { *err_ = why; return B200MIX_ERR_INVALID; }
-    int fail(const char *what, cudaError_t e)
-    { *err_ = std::string(what) + ": " + cudaGetErrorString(e); return B200MIX_ERR_CUDA; }
 
     // A new array holding `count` elements of host memory, copied on the stream: the setter's
     // commit() waits for the copy, so the source must live until then.
@@ -368,7 +362,7 @@ private:
     template<typename Part>
     int commit(Part &part, Part &next)
     {
-        OUT_TRY(cudaStreamSynchronize(s_));
+        CUDA_TRY(*err_, cudaStreamSynchronize(s_));
         part = std::move(next);
         return B200MIX_OK;
     }
@@ -385,6 +379,5 @@ private:
     size_t out_bytes_{0};
 };
 
-#undef OUT_TRY
 
 } // namespace b200mix

@@ -36,7 +36,7 @@ struct VoiceBook {
     std::vector<uint32_t> send_slot;               // [voice][num_sends]
     std::vector<uint32_t> bufrefs;                 // active static voices per buffer
     uint32_t voice_hi{0};                          // 1 + highest voice index ever set
-    bool dry_active{false};                        // a voice or an effect slot has fed the dry bus
+    bool dry_active{false};                        // a voice has fed the dry bus
     bool dev_filters{false};                       // filter activity is decided on the device
 
     std::vector<uint32_t> order, order2, slot_start;

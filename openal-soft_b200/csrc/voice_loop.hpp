@@ -18,9 +18,6 @@
 
 namespace b200mix {
 
-// Every call below returns a B200MIX_* code and, when it fails, sets the device's error string.
-#define LOOP_TRY(expr) do { const cudaError_t e_ = (expr); if(e_ != cudaSuccess) return fail(#expr, e_); } while(0)
-
 class VoiceLoop {
 public:
     // The kernels and their grids' limits, the partial rows, and what a parking device or one with
@@ -30,7 +27,7 @@ public:
         float *dry_cur, const float *dry_tgt, float *send_cur, const float *send_tgt)
     {
         dd_ = dd; num_sms_ = num_sms; s_ = stream; err_ = &err;
-        LOOP_TRY(order_.alloc(dd.max_voices, s_));
+        CUDA_TRY(*err_, order_.alloc(dd.max_voices, s_));
         // non-HRTF devices with <= 4 dry channels mix the dry bus in registers; HRTF devices and
         // wider dry mixes resample + park (k_hrtf_fir mixes the HRTF voices, the parked dry bus
         // the others)
@@ -38,23 +35,23 @@ public:
         cdr_ = !hrtfDev && dd.dry_channels <= 4 ? 4 : 0;
         mix_fn_ = cdr_ ? k_mix_voices<kMixGS, kMixGroups, 4> : k_mix_voices<kMixGS, kMixGroups, 0>;
         mix_smem_ = (cdr_ ? sizeof(GroupSmem<4>) : sizeof(GroupSmem<0>))*kMixGroups;
-        LOOP_TRY(cudaFuncSetAttribute(mix_fn_, cudaFuncAttributeMaxDynamicSharedMemorySize, int(mix_smem_)));
+        CUDA_TRY(*err_, cudaFuncSetAttribute(mix_fn_, cudaFuncAttributeMaxDynamicSharedMemorySize, int(mix_smem_)));
         int perSm = 0;
-        LOOP_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, mix_fn_, kMixGS*kMixGroups, mix_smem_));
+        CUDA_TRY(*err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, mix_fn_, kMixGS*kMixGroups, mix_smem_));
         mix_blocks_per_sm_ = std::max(perSm, 1);
         if(parks_dry())
         {
             // the parking variant writes every mixed voice's line and state bits
             if(int rc = ensure_park_lines()) return rc;
-            LOOP_TRY(claim_.alloc(2, s_));
+            CUDA_TRY(*err_, claim_.alloc(2, s_));
         }
         if(hrtfDev)
         {
             // 17 outputs per thread / 64 front pad for ir <= 64, 19 / 128 for ir <= 128
             fir_fn_ = dd.ir_size <= 64u ? k_hrtf_fir<17, 64> : k_hrtf_fir<19, 128>;
             fir_smem_ = (dd.ir_size <= 64u ? sizeof(FirSmem<kFirGS, 17, 64>) : sizeof(FirSmem<kFirGS, 19, 128>))*kFirGroups;
-            LOOP_TRY(cudaFuncSetAttribute(fir_fn_, cudaFuncAttributeMaxDynamicSharedMemorySize, int(fir_smem_)));
-            LOOP_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, fir_fn_, kFirGS*kFirGroups, fir_smem_));
+            CUDA_TRY(*err_, cudaFuncSetAttribute(fir_fn_, cudaFuncAttributeMaxDynamicSharedMemorySize, int(fir_smem_)));
+            CUDA_TRY(*err_, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, fir_fn_, kFirGS*kFirGroups, fir_smem_));
             // the FIR grid sets the partial rows, hence the summation order: it is fixed at
             // kFirCtasPerSm per SM (the launch bounds), not at whatever more might fit
             fir_blocks_per_sm_ = std::max(std::min(perSm, kFirCtasPerSm), 1);
@@ -63,7 +60,7 @@ public:
         // rows in two regions, k_mix_voices' and k_mix_deferred's (voices with direct filters)
         partial_floats_ = hrtfDev ? size_t(num_sms_)*fir_blocks_per_sm_*(2*kAccumLen)
             : size_t(num_sms_)*mix_blocks_per_sm_*size_t(cdr_)*kLine;
-        LOOP_TRY(partial_.alloc(std::max<size_t>((hrtfDev ? 1 : 2)*partial_floats_, 4), s_));
+        CUDA_TRY(*err_, partial_.alloc(std::max<size_t>((hrtfDev ? 1 : 2)*partial_floats_, 4), s_));
 
         // a CTA's 8 warps share its entries evenly: chunks of 64 dry entries (128 per send slot) keep
         // the first (fading) tile's serial work per warp short
@@ -99,7 +96,7 @@ public:
         if(int rc = ensure_park_lines()) return rc;
         const bool wide = dd_.dry_channels > 4u && dd_.dry_channels <= uint32_t(kPmN);
         if(wide)
-            LOOP_TRY(cudaFuncSetAttribute(k_panmix_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, kPmStages*kPmStageBytes + 1024));
+            CUDA_TRY(*err_, cudaFuncSetAttribute(k_panmix_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, kPmStages*kPmStageBytes + 1024));
         if(int rc = alloc(dry_, dd_.max_voices)) return rc;
         // B200MIX_PANMIX_SIMT=1 keeps the whole pan-mix on k_send_mix (A/B measurements only)
         const char *simt = std::getenv("B200MIX_PANMIX_SIMT");
@@ -114,8 +111,8 @@ public:
         if(int rc = ensure_park_lines()) return rc;
         const size_t gains = size_t(dd_.max_voices)*dd_.real_channels;
         DevArray<float> cur, tgt;
-        LOOP_TRY(cur.alloc(gains, s_));
-        LOOP_TRY(tgt.alloc(gains, s_));
+        CUDA_TRY(*err_, cur.alloc(gains, s_));
+        CUDA_TRY(*err_, tgt.alloc(gains, s_));
         if(int rc = alloc(real_, dd_.max_voices)) return rc;
         real_.cur = cur; real_.tgt = tgt;
         real_cur_ = std::move(cur); real_tgt_ = std::move(tgt);
@@ -127,8 +124,8 @@ public:
     {
         if(qhdr_) return B200MIX_OK;
         DevArray<uint4> qhdr; DevArray<uint32_t> queue;
-        LOOP_TRY(qhdr.alloc(dd_.max_voices, s_));
-        LOOP_TRY(queue.alloc(size_t(dd_.max_voices)*kMaxQueue, s_));
+        CUDA_TRY(*err_, qhdr.alloc(dd_.max_voices, s_));
+        CUDA_TRY(*err_, queue.alloc(size_t(dd_.max_voices)*kMaxQueue, s_));
         qhdr_ = std::move(qhdr); queue_ = std::move(queue);
         return B200MIX_OK;
     }
@@ -140,11 +137,11 @@ public:
         const size_t count = size_t(dd_.max_voices)*paths();
         if(int rc = ensure_park_lines()) return rc;
         DevArray<FilterRec> filt; DevArray<float> dline; DevArray<uint32_t> order2;
-        LOOP_TRY(filt.alloc(count));
-        LOOP_TRY(dline.alloc(size_t(dd_.max_voices)*kLine, s_));
-        LOOP_TRY(order2.alloc(dd_.max_voices, s_));
+        CUDA_TRY(*err_, filt.alloc(count));
+        CUDA_TRY(*err_, dline.alloc(size_t(dd_.max_voices)*kLine, s_));
+        CUDA_TRY(*err_, order2.alloc(dd_.max_voices, s_));
         k_filter_init<<<unsigned((count*32u + 255u)/256u), 256, 0, s_>>>(filt, count);
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
         ++launches;
         filt_ = std::move(filt); dline_ = std::move(dline); order2_ = std::move(order2);
         return B200MIX_OK;
@@ -160,15 +157,15 @@ public:
     // b200mix_voices_filters' updates, once ensure_filters has run.
     int set_filters(uint32_t n, const FilterUpdate *updates, uint64_t &launches)
     {
-        LOOP_TRY(fstage_.wait());
+        CUDA_TRY(*err_, fstage_.wait());
         const size_t cap = std::max<size_t>(n, 2u*fstage_.capacity());
-        LOOP_TRY(fstage_.reserve(n, cap, cap*sizeof(FilterUpdate), cap*sizeof(FilterUpdate), s_));
+        CUDA_TRY(*err_, fstage_.reserve(n, cap, cap*sizeof(FilterUpdate), cap*sizeof(FilterUpdate), s_));
         fstage_.begin();
         const FilterUpdate *fupd = fstage_.pack(updates, n);
-        LOOP_TRY(fstage_.ship(s_));
+        CUDA_TRY(*err_, fstage_.ship(s_));
         k_apply_filter_updates<<<(2u*n + 127u)/128u, 128, 0, s_>>>(filt_, paths(), fupd, n);
         ++launches;
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
         return B200MIX_OK;
     }
 
@@ -178,7 +175,7 @@ public:
         if(int rc = ensure_queues()) return rc;
         k_set_queue<<<1, 32, 0, s_>>>(voices, qhdr_, queue_, Q);
         ++launches;
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
         return B200MIX_OK;
     }
 
@@ -209,8 +206,8 @@ public:
     int launch(MixParams P, const VoiceBook &B, float *dry, float *real, float *wet, uint64_t &launches,
         Mark &&mark)
     {
-        if(pending_.order) { LOOP_TRY(b200mix::upload(order_, B.order, s_)); pending_.order = false; }
-        if(pending_.order2) { LOOP_TRY(b200mix::upload(order2_, B.order2, s_)); pending_.order2 = false; }
+        if(pending_.order) { CUDA_TRY(*err_, b200mix::upload(order_, B.order, s_)); pending_.order = false; }
+        if(pending_.order2) { CUDA_TRY(*err_, b200mix::upload(order2_, B.order2, s_)); pending_.order2 = false; }
         if(pending_.dry) { if(int rc = upload(dry_, B.dry_entries, nullptr)) return rc; pending_.dry = false; }
         if(pending_.sends) { if(int rc = upload(sends_, B.entries, &B.slot_start)) return rc; pending_.sends = false; }
         if(pending_.real && real_.entries)
@@ -226,7 +223,7 @@ public:
         mark(1);
         mix_fn_<<<blocks, kMixGS*kMixGroups, mix_smem_, s_>>>(P);
         ++launches;
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
         const uint64_t mixDone = launches;
 
         mark(2);
@@ -252,7 +249,7 @@ public:
                     sizeof(DeferredSmem<kMixGroups, 4>), s_>>>(P2);
                 ++launches;
             }
-            LOOP_TRY(cudaGetLastError());
+            CUDA_TRY(*err_, cudaGetLastError());
         }
         // the HRIR FIR's partial rows are summed by the HRTF post-process (OutputStage::post)
         fir_rows_ = 0;
@@ -261,7 +258,7 @@ public:
             fir_rows_ = std::max(1u, std::min(uint32_t(num_sms_*fir_blocks_per_sm_), (numOrder + kFirGroups - 1)/kFirGroups));
             // straight behind the resample kernel (no direct filters in between), its set-up runs
             // under the resample kernel's last CTAs
-            LOOP_TRY(launch_ex(s_, launches, launches == mixDone, fir_fn_, dim3(fir_rows_), dim3(kFirGS*kFirGroups),
+            CUDA_TRY(*err_, launch_ex(s_, launches, launches == mixDone, fir_fn_, dim3(fir_rows_), dim3(kFirGS*kFirGroups),
                 fir_smem_, P));
             fir_done_ = launches;
         }
@@ -272,7 +269,7 @@ public:
         for(uint32_t r = 0;r < 2 && !parks_dry() && rows[r];++r, ++launches)
             k_reduce_rows<<<(len/4 + kReduceCols - 1)/kReduceCols, 1024, 0, s_>>>(partial_ + r*partial_floats_, rows[r],
                 len, dry, 1);
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
 
         mark(4);
         // ---- parked dry bus: non-HRTF voices of the parking variant ----
@@ -326,16 +323,13 @@ private:
 
     uint32_t paths() const { return 1u + dd_.num_sends; }
 
-    int fail(const char *what, cudaError_t e)
-    { *err_ = std::string(what) + ": " + cudaGetErrorString(e); return B200MIX_ERR_CUDA; }
-
     // Parked lines and state bits of every voice (the resample kernel writes them, buses and filters read them).
     int ensure_park_lines()
     {
         if(xscratch_) return B200MIX_OK;
         DevArray<float> xscratch; DevArray<uint32_t> sendinfo;
-        LOOP_TRY(xscratch.alloc(size_t(dd_.max_voices)*kLine, s_));
-        LOOP_TRY(sendinfo.alloc(dd_.max_voices, s_));
+        CUDA_TRY(*err_, xscratch.alloc(size_t(dd_.max_voices)*kLine, s_));
+        CUDA_TRY(*err_, sendinfo.alloc(dd_.max_voices, s_));
         xscratch_ = std::move(xscratch); sendinfo_ = std::move(sendinfo);
         return B200MIX_OK;
     }
@@ -344,10 +338,10 @@ private:
     int alloc(Bus &b, size_t count)
     {
         DevArray<SendEntry> entries; DevArray<uint32_t> slotStart; DevArray<float> geff; DevArray<float4> gramp;
-        LOOP_TRY(entries.alloc(count, s_));
-        LOOP_TRY(slotStart.alloc(b.slots + 1, s_));
-        LOOP_TRY(geff.alloc(count*b.cw, s_));
-        LOOP_TRY(gramp.alloc(count*b.cw, s_));
+        CUDA_TRY(*err_, entries.alloc(count, s_));
+        CUDA_TRY(*err_, slotStart.alloc(b.slots + 1, s_));
+        CUDA_TRY(*err_, geff.alloc(count*b.cw, s_));
+        CUDA_TRY(*err_, gramp.alloc(count*b.cw, s_));
         b.entries = std::move(entries); b.slot_start = std::move(slotStart);
         b.geff = std::move(geff); b.gramp = std::move(gramp);
         return B200MIX_OK;
@@ -361,8 +355,8 @@ private:
         if(a.size() >= need) return B200MIX_OK;
         count = std::max(count, need);
         DevArray<T> next;
-        LOOP_TRY(zero ? next.alloc(count, s_) : next.alloc(count));
-        LOOP_TRY(cudaStreamSynchronize(s_));
+        CUDA_TRY(*err_, zero ? next.alloc(count, s_) : next.alloc(count));
+        CUDA_TRY(*err_, cudaStreamSynchronize(s_));
         a = std::move(next);
         return B200MIX_OK;
     }
@@ -372,9 +366,9 @@ private:
     int upload(Bus &b, const std::vector<SendEntry> &entries, const std::vector<uint32_t> *slot_start)
     {
         const uint32_t ss[2] = {0u, uint32_t(entries.size())};
-        if(slot_start) LOOP_TRY(b200mix::upload(b.slot_start, *slot_start, s_));
-        else LOOP_TRY(cudaMemcpyAsync(b.slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, s_));
-        LOOP_TRY(b200mix::upload(b.entries, entries, s_));
+        if(slot_start) CUDA_TRY(*err_, b200mix::upload(b.slot_start, *slot_start, s_));
+        else CUDA_TRY(*err_, cudaMemcpyAsync(b.slot_start, ss, sizeof(ss), cudaMemcpyHostToDevice, s_));
+        CUDA_TRY(*err_, b200mix::upload(b.entries, entries, s_));
         return B200MIX_OK;
     }
 
@@ -412,7 +406,7 @@ private:
             ++launches;
         }
         if(num_entries) { k_send_gains_update<<<gainGrid, 128, 0, s_>>>(M, num_entries); ++launches; }
-        LOOP_TRY(cudaGetLastError());
+        CUDA_TRY(*err_, cudaGetLastError());
         return B200MIX_OK;
     }
 
@@ -444,6 +438,5 @@ private:
     uint32_t frames_{0}; bool mix_sends_{false}, real_mixed_{false};   // this update's (prepare)
 };
 
-#undef LOOP_TRY
 
 } // namespace b200mix

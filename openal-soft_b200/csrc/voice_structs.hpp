@@ -14,10 +14,9 @@ struct ConvRing {
     uint32_t nb_last, f_last, cur_last;        // last update: blocks completed, fill and position at its start
 };
 
-// One effect slot as the kernels see it.  The host writes every field (b200mix.cu, from
-// SlotTable); what a kernel carries from one update to the next lives behind the pointers
-// (ring, H, lines, gains), so the host may upload any record at any time without overwriting
-// device state.
+// One effect slot as the kernels see it.  The host writes every field (SlotTable); what a kernel
+// carries from one update to the next lives behind the pointers (ring, H, lines, gains), so the
+// host may upload any record at any time without overwriting device state.
 struct SlotRec {
     uint32_t type, channels, frames, segs;     // type: b200mix_effect; segs = mNumConvolveSegs
     uint32_t rv_cur, rv_mask;                  // reverb: current pipeline object; objects to run now

@@ -56,7 +56,7 @@ def nseg(taps):
 # ---- the host's chunk plan ---------------------------------------------------------------
 
 def conv_chunks(slots, sms):
-    """SlotTable::refresh (csrc/slot_table.hpp:93-98): slots = [(segs, channels)] of the
+    """SlotTable::refresh (csrc/slot_table.hpp:445-450): slots = [(segs, channels)] of the
     installed convolution slots."""
     work = sum(ch for _, ch in slots)
     segs = max(s for s, _ in slots)

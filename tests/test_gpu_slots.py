@@ -6,7 +6,9 @@
 - Disable: from the next update on, a device renders (and launches) what a device that never had
   the slot does.
 - Re-install: one slot taken through every kind of effect without a render in between renders (and
-  launches) what a fresh device with only the last install does."""
+  launches) what a fresh device with only the last install does.
+- A refused slot call changes nothing: after it, the device renders (and launches) what its twin that
+  never made the call does, and it reports the refusal's code and message."""
 import ctypes as C
 
 import numpy as np
@@ -144,3 +146,86 @@ def test_reinstall_through_every_kind_equals_fresh_install():
     assert np.abs(np.concatenate(fresh_out, axis=1)).max() > 1e-4
     for a, b in zip(chain_out, fresh_out):
         assert np.array_equal(a, b)
+
+
+ERR_INVALID = -1
+
+
+def _reverb_params(**changes):
+    fx = golden.load("hrtf_bsinc24_reverb_v6")
+    params = abi.reverb_params_from(fx["reverb_params"].tobytes())
+    for k, v in changes.items():
+        setattr(params, k, v)
+    params.struct_size = C.sizeof(abi.ReverbParams)
+    return params, fx["reverb_gains"]
+
+
+def _raw_efx(dev, slot, out_channels=4, struct_size=None):
+    """b200mix_slot_efx with an echo and maps of `out_channels` outputs; its return code."""
+    props = abi.efx_defaults(abi.EFFECT_ECHO)
+    props.struct_size = C.sizeof(abi.EfxProps) if struct_size is None else struct_size
+    scale, index = np.ones(out_channels, dtype=np.float32), np.arange(out_channels, dtype=np.uint32)
+    t = abi.EfxTarget()
+    t.struct_size, t.sample_rate, t.slot_gain = C.sizeof(abi.EfxTarget), dev.desc.sample_rate, 0.7
+    t.out_channels, t.out_scale, t.out_index = out_channels, scale.ctypes.data, index.ctypes.data
+    t.wet_channels, t.wet_index = len(INDEX), INDEX.ctypes.data
+    t.real_center, t.real_lfe, t.device_ambi_order = abi.NO_SLOT, abi.NO_SLOT, 1
+    return dev.m.slot_efx(dev.h, slot, C.byref(props), C.byref(t))
+
+
+def _raw_gains(dev, slot, lines):
+    g = np.ones((lines, 4), dtype=np.float32)
+    return dev.m.slot_output_gains(dev.h, slot, lines, g.ctypes.data)
+
+
+# (call, the refusal's message); slots: 0 convolution, 1 reverb mid-fade, 2 echo into slot 1, 3 empty
+REFUSED = {
+    "disable_out_of_range": (lambda dev: dev.m.slot_disable(dev.h, 4), "slot_disable: bad slot"),
+    "convolution_17_channels": (
+        lambda dev: dev.m.slot_convolution(dev.h, 0, 17, 64, np.ones((17, 64), dtype=np.float32).ctypes.data),
+        "slot_convolution: bad arguments (or the device has no sends/slots)"),
+    "reverb_line_not_pow2": (
+        lambda dev: dev.m.slot_reverb(dev.h, 1, C.byref(_reverb_params(late_len=3000)[0])),
+        "slot_reverb: line lengths must be powers of two, feedback delays non-zero"),
+    "reverb_update_other_lengths": (
+        lambda dev: dev.m.slot_reverb_update(dev.h, 1, C.byref(_reverb_params(main_len=65536)[0]), 1),
+        "slot_reverb_update: line lengths differ from the installed ones"),
+    "reverb_update_on_echo": (
+        lambda dev: dev.m.slot_reverb_update(dev.h, 2, C.byref(_reverb_params()[0]), 0),
+        "slot_reverb_update: no reverb installed on this slot / bad arguments"),
+    "efx_maps_mismatch": (lambda dev: _raw_efx(dev, 2, out_channels=3),
+                          "slot_efx: the target maps do not match the device's wet / output mix"),
+    "efx_struct_size": (lambda dev: _raw_efx(dev, 2, struct_size=C.sizeof(abi.EfxProps) - 4),
+                        "slot_efx: bad arguments (or the device has no sends/slots)"),
+    "target_loop": (lambda dev: dev.m.slot_target(dev.h, 1, 2), "slot_target: the chain would loop"),
+    "output_gains_line_count": (lambda dev: _raw_gains(dev, 1, 7), "slot_output_gains: wrong line count"),
+    "output_gains_empty_slot": (lambda dev: _raw_gains(dev, 3, 2), "slot_output_gains: bad arguments"),
+}
+
+
+@pytest.mark.parametrize("case", sorted(REFUSED))
+def test_rejected_slot_call_changes_nothing(case):
+    call, message = REFUSED[case]
+    desc = _post_none_desc(4)
+    runs = []
+    for refuse in (True, False):
+        dev, voices = _device(desc, seed=53)
+        _conv(dev, 0)                              # 5000 taps
+        _reverb(dev, 1, 0)
+        dev.slot_target(2, 1)
+        _echo(dev, 2)
+        dev.voices_update(*voices)
+        _render(dev, (512,))
+        params, gains = _reverb_params(fade_samples=4000)
+        dev.slot_reverb_update(1, params, True, gains)
+        _render(dev, (700,))                       # the reverb is mid-fade
+        if refuse:
+            assert call(dev) == ERR_INVALID
+            assert dev.last_error() == message
+        runs.append(_render(dev, SIZES[1:6]))
+        dev.close()
+    (refused_out, refused_n), (twin_out, twin_n) = runs
+    assert refused_n == twin_n
+    assert np.abs(np.concatenate(twin_out, axis=1)).max() > 1e-4
+    for a, b in zip(refused_out, twin_out):
+        assert a.tobytes() == b.tobytes()
